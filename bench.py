@@ -1,13 +1,19 @@
 #!/usr/bin/env python
 """Benchmark of the NoisyNet hot path: CIFAR-10 4-bit NoisyNet (I_max = 1 nA) training images/sec.
 
-    python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path
+    python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a path
     python bench.py --impl reference --steps K --warmup W    # the reference's CPU path (oracle port)
+    python bench.py ... --dump-outputs DIR                    # also write what the last timed step computed (.npy)
 
 A "step" = one full training step (forward, loss, backward, AdamW, weight clamp -- noisynet.py:1276-1542)
 over one batch of synthetic CIFAR-10-shaped 4-bit data (random-init weights; no dataset on disk).
 Workload = BASELINE.json configs[1]: NoisyNet, --current 1 --act_max 5 --w_max1 0.3, --q_a 4 --q_w 4,
 batch 512 per GPU.  One JSON line on stdout (rank 0).
+
+--dump-outputs DIR writes, right after the timed steps, what the timed path handed back in its last step: the loss
+(loss.npy) and the model state it updated in place (state.<name>.npy: parameters and BatchNorm running statistics),
+float32, about 6 MB.  Inputs, weights and random streams are seeded, so two builds run with the same arguments can be
+compared output for output.
 """
 import argparse
 import json
@@ -19,6 +25,7 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 FLOP_FWD = {"conv1": 15.288e6, "conv2": 78.0e6, "fc1": 4.68e6, "fc2": 0.0156e6}   # main + sigma^2, per image
@@ -43,6 +50,8 @@ def parse():
     p.add_argument("--cpu-baseline-seconds", type=float, default=12.0)
     p.add_argument("--no-cpu-baseline", action="store_true")
     p.add_argument("--pool", type=int, default=24, help="distinct resident input batches cycled through")
+    p.add_argument("--dump-outputs", default=None, metavar="DIR",
+                   help="write the loss and the updated model state of the last timed step as DIR/<name>.npy (library path)")
     return p.parse_args()
 
 
@@ -52,7 +61,8 @@ def load_peaks():
             d = json.load(f)
         return d, "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # NVIDIA's H100 SXM data sheet (700 W card, dense bf16): not reached in practice
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "data sheet"
 
 
 class ClockSampler(threading.Thread):
@@ -146,7 +156,7 @@ def oracle_arm(batch, variant, steps, warmup, seconds=None):
 
 
 def torch_gpu_arm(batch, variant, steps, warmup, dev):
-    """The bar SURVEY.md section 2.2 / BASELINE.md section 3 name: the reference's step in PyTorch-eager on the SAME B200
+    """The bar SURVEY.md section 2.2 / BASELINE.md section 3 name: the reference's step in PyTorch-eager on the SAME GPU
     (cuDNN / cuBLAS contractions, ATen elementwise + Philox kernels, torch.optim.AdamW) -- the oracle port of the reference
     step moved to the GPU unchanged, inputs resident on the device, timed with CUDA events.  Not the product path."""
     from oracle import noisynet_oracle as O
@@ -187,7 +197,7 @@ def run_torch_gpu(args):
         "n_gpus": 1, "steps": r["steps"], "warmup": max(args.warmup, 3), "ms_per_step": r["ms_per_step"],
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": workload_config(args, 1), "final_loss": r["final_loss"],
-        "note": "PyTorch-eager (cuDNN/cuBLAS/ATen) run of the reference step (oracle port) on one B200: the library bar",
+        "note": "PyTorch-eager (cuDNN/cuBLAS/ATen) run of the reference step (oracle port) on one GPU: the library bar",
     }
     print(json.dumps(line), flush=True)
 
@@ -213,7 +223,7 @@ def workload_config(args, world):
     return {"workload": "NoisyNet CIFAR-10 (conv5x5x65 - conv5x5x120 - fc390 - fc10), I_max=1nA all layers, act_max=5, w_max1=0.3, "
                         + ("q_a=4 q_w=4 stochastic rounding" if args.variant == "q4" else "README flags (q_a=q_w=0)"),
             "per_gpu_batch": args.batch, "global_batch": args.batch * world, "parallelism": "dp%d" % world,
-            "flow": args.flow, "l2_policy": "inputs+activations (>400 MB/step) exceed the 126 MB L2; %d distinct input batches cycled" % args.pool}
+            "flow": args.flow, "l2_policy": "inputs+activations (>400 MB/step) exceed the 50 MB L2; %d distinct input batches cycled" % args.pool}
 
 
 # ------------------------------------------------------------------------------------ our arm
@@ -290,7 +300,7 @@ def time_second_variant(args, dev, precision, variant):
 
 
 def pick_precision(args, dev):
-    """auto: the tcgen05 path (bf16 integer codes for q4, tf32 otherwise) if it passes a self-check, else fp32."""
+    """auto: the tensor-core path (bf16 operands: exact integer codes for q4) if it passes a self-check, else fp32."""
     if args.precision != "auto":
         return args.precision
     from noisynet_b200 import ops
@@ -307,7 +317,7 @@ def pick_precision(args, dev):
         if (y0 - y1).abs().max().item() < 5e-2 * y0.abs().max().item():
             return want
     except Exception as e:  # noqa: BLE001
-        sys.stderr.write("[bench] tcgen05 path unavailable (%s); using fp32 CUDA-core kernels\n" % e)
+        sys.stderr.write("[bench] tensor-core path unavailable (%s); using fp32 CUDA-core kernels\n" % e)
     return "fp32"
 
 
@@ -339,7 +349,7 @@ def run_b200(args):
     engine = None
     if args.flow == "engine":
         if not (fused_opt and precision == "bf16"):
-            raise SystemExit("--flow engine needs the tcgen05 path (bf16) and --optimizer fused")
+            raise SystemExit("--flow engine needs the tensor-core path (bf16) and --optimizer fused")
         from noisynet_b200.engine import NoisyNetEngine
         engine = NoisyNetEngine(model, B, opt=opt, reducer=red if world > 1 else None)
 
@@ -421,6 +431,8 @@ def run_b200(args):
     ms = t_ms.item()
     value = world * B * args.steps / (ms * 1e-3)
     final_loss = loss_out.item()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss_out, model)
 
     # ---------------- timed region 2: end to end through the public API with HOST buffers ("e2e")
     # Every step's input travels host (pinned) -> device inside the timed region; the copy of step i+1 is issued
@@ -497,7 +509,7 @@ def run_b200(args):
         w_eff = ops.quantize_fwd(w_raw, 4, -1.0, 1.0, 0.0) if args.variant == "q4" else w_raw
         scale = ops.tensor_stats(xs[0])[0:1]
         reps = 20
-        # CUDA events bracket the main tcgen05 kernel only, on its launch stream (nn_debug_main_kernel_ms); the
+        # CUDA events bracket the main tensor-core kernel only, on its launch stream (nn_debug_main_kernel_ms); the
         # operand packs that precede it in this standalone call are not part of the engine's step.
         call = lambda i: ops.noisy_conv_fwd(xs[i % 8], w_eff, w_raw, None, 1, 0, noise_mode=NOISE_EXTERNAL, current=1.0,
                                             scale_dev=scale, precision=precision, want_y=False,
@@ -520,23 +532,15 @@ def run_b200(args):
                 tms.append(lib.nn_debug_main_kernel_ms(-1))
             lib.nn_debug_main_kernel_ms(0)
             k_ms = sum(tms) / len(tms)
-        traffic = None
-        try:
-            with open(os.path.join(ROOT, "profiles", "r2_conv2_fwd_traffic.json")) as f:
-                tj = json.load(f)
-                traffic = {"dram_bytes_per_launch": tj["dram_bytes_per_launch"], "l2_to_sm_bytes_per_launch": tj["l2_to_sm_bytes"],
-                           "unit": "B", "from": tj["source"]} if (B == 512 and precision == "bf16") else None
-        except Exception:
-            traffic = None
         flops = FLOP_FWD["conv2"] * B
         achieved = flops / (k_ms * 1e-3) / 1e12
-        peak = peaks.get("bf16_tflops", 1590.0)
-        roof = {"kernel": "k_conv_tma<1>: fused noisy conv forward of conv2 (M=%d, N=2x120, K=1625; persistent CTA pairs, "
+        peak = peaks.get("bf16_tflops", 989.0)
+        roof = {"kernel": "k_conv_tma<1>: fused noisy conv forward of conv2 (M=%d, N=2x120, K=1625; persistent CTAs, wgmma, "
                           "TMA-im2col operands), precision=%s" % (B * 100, precision),
                 "bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                "peak_kind": peak_kind + " (burst, kernel timed alone)", "kernel_ms": k_ms,
-                "flop_per_launch": flops, "traffic": traffic,
-                "step_tensor_frac": (world * B * args.steps / (ms * 1e-3)) * FLOP_STEP / world / (peaks.get("bf16_tflops_sustained", 1400.0) * 1e12)}
+                "peak_kind": peak_kind + " (kernel timed alone)", "kernel_ms": k_ms,
+                "flop_per_launch": flops,
+                "step_tensor_frac": (world * B * args.steps / (ms * 1e-3)) * FLOP_STEP / world / (peaks.get("bf16_tflops_sustained", 989.0) * 1e12)}
 
     if rank != 0:
         return
@@ -578,8 +582,23 @@ def run_b200(args):
     print(json.dumps(line), flush=True)
 
 
+def dump_outputs(out_dir, loss, model):
+    """loss.npy + state.<name>.npy (float32) of the step that just ran: what a caller of the training step receives."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": loss.detach().float().reshape(-1)}
+    for k, v in model.state_dict().items():
+        if torch.is_floating_point(v):
+            arrays["state." + k] = v.detach().float()
+    total = sum(a.numel() * 4 for a in arrays.values())
+    assert total <= 64 << 20, "dump of %d bytes exceeds 64 MB" % total
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a.cpu().numpy().astype(np.float32))
+
+
 def main():
     args = parse()
+    if args.dump_outputs and args.impl != "b200":
+        raise SystemExit("--dump-outputs is implemented for the library path (--impl b200)")
     if args.impl == "reference":
         run_reference(args)
     elif args.impl == "torch_gpu":

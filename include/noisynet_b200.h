@@ -1,5 +1,5 @@
 /*
- * noisynet_b200 -- C ABI of the B200 (sm_100a) NoisyNet hot path.
+ * noisynet_b200 -- C ABI of the H100 (sm_90a) NoisyNet hot path.
  *
  * The reference (michaelklachko/NoisyNet) is pure Python on PyTorch and has no FFI of its
  * own; its "operator API" for this path is the set of Python names the drivers import
@@ -40,7 +40,7 @@ const char* nn_last_error(void);
 int nn_abi_version(void);
 /* number of kernels this library has launched in this process (host-side counter). */
 uint64_t nn_launch_count(void);
-/* sm_count / compute capability of `device`; fails unless the device is sm_100. */
+/* sm_count / compute capability of `device`; fails unless the device is sm_90 (H100). */
 int nn_device_info(int device, int* sm_count, int* cc_major, int* cc_minor);
 /* *offset_dev += inc (one thread); graph-capturable. */
 int nn_rng_advance(uint64_t* offset_dev, uint64_t inc, int device, void* stream);
@@ -136,8 +136,8 @@ typedef struct nn_conv_geom {
 
 enum { NN_NOISE_NONE = 0, NN_NOISE_MERGED = 1, NN_NOISE_EXTERNAL = 2 };
 enum { NN_PREC_FP32 = 0,      /* CUDA-core fp32 FMA (reference arithmetic, any geometry)  */
-       NN_PREC_TF32 = 1,      /* tcgen05 kind::tf32, fp32 accumulate in TMEM              */
-       NN_PREC_BF16 = 2 };    /* tcgen05 kind::f16 (bf16), fp32 accumulate; exact when the
+       NN_PREC_TF32 = 1,      /* reserved: rejected (not implemented)                     */
+       NN_PREC_BF16 = 2 };    /* wgmma bf16 x bf16, fp32 accumulate; exact when the      
                                  operands are integer codes (a_code_scale > 0)             */
 
 typedef struct nn_conv_fwd_args {
@@ -169,7 +169,7 @@ typedef struct nn_conv_fwd_args {
     float a_code_scale, w_code_scale;
     void* workspace;         /* device scratch for packed operands (nn_conv_workspace_bytes) */
     int64_t workspace_bytes;
-    const void* x_packed;    /* optional (tcgen05 precisions): the input already packed as NHWC bf16
+    const void* x_packed;    /* optional (tensor-core precisions): the input already packed as NHWC bf16
                                 [B,H,W,ceil8(Cin)] (codes if a_code_scale > 0), e.g. by nn_stage_fwd;
                                 `x` is then ignored and the pack kernel is skipped                    */
     const void* w_packed;    /* optional: weights already packed by nn_prepare_weights (mode 0, same
@@ -221,15 +221,15 @@ int nn_debug_shift_enable(int enable);
 
 int64_t nn_conv_workspace_bytes(const nn_conv_geom* g, int32_t precision);
 /* 1 if (geometry, precision) is served for which = 0 forward / 1 dgrad / 2 wgrad.  NN_PREC_FP32 serves
- * everything; the tcgen05 precisions serve a subset (callers pick NN_PREC_FP32 for the rest). */
+ * everything; the tensor-core precisions serve a subset (callers pick NN_PREC_FP32 for the rest). */
 int nn_conv_supported(const nn_conv_geom* g, int32_t precision, int32_t which);
-/* Test/debug hook: synchronises `device` and returns the tcgen05 pipeline watchdog flag (0 = ok);
+/* Test/debug hook: synchronises `device` and returns the tensor-core pipeline watchdog flag (0 = ok);
  * reset != 0 clears it. */
 int nn_debug_error_flag(int device, int reset);
-/* Measurement hook: enable = 1/0 brackets the main tcgen05 forward kernel (not the operand packs) with CUDA
+/* Measurement hook: enable = 1/0 brackets the main tensor-core forward kernel (not the operand packs) with CUDA
  * events on its launch stream; enable < 0 synchronises on them and returns the last elapsed ms (-1: none). */
 float nn_debug_main_kernel_ms(int enable);
-/* Debug (env NN_UMMA_DEBUG=1): per-CTA clock64 phase stamps [cta][8] of the last tcgen05 forward launch. */
+/* Debug (env NN_UMMA_DEBUG=1): per-CTA clock64 phase stamps [cta][8] of the last tensor-core forward launch. */
 int nn_debug_cta_timeline(long long* host_out, int max_ctas);
 int nn_noisy_conv_fwd(const nn_conv_fwd_args* a, int device, void* stream);
 
@@ -279,7 +279,7 @@ int64_t nn_conv_gy_planes_bytes(const nn_conv_geom* g);
 int nn_noisy_conv_wgrad(const nn_conv_wgrad_args* a, int device, void* stream);
 
 /* ---- weight preparation for a whole step in one launch ------------------------------------------------
- * Each job packs one layer's weights into the tcgen05 operand image: mode 0 = forward rows
+ * Each job packs one layer's weights into the tensor-core operand image: mode 0 = forward rows
  * [quantized main | g(|w_raw|) | colsum |w_raw|], mode 1 = transposed, tap-flipped rows for dgrad.  With
  * q_bits > 0 the weight quantizer (hardware_model.py:323, :343: range [-q_hi, q_hi], stochastic rounding)
  * runs in registers; jobs sharing `rng` (or u_inject) quantize identically.  `jobs` is a HOST array (<= 8). */
@@ -305,7 +305,7 @@ int nn_prepare_weights(const nn_wprep_job* jobs, int count, int device, void* st
 /* ---- section 8f.1: the between-layer stages, fused ---------------------------------------------------
  * conv stage (noisynet.py:419-460, 483-520): MaxPool2d(2,2) -> BatchNorm (batch statistics, running stats
  * updated) -> ReLU -> clamp(max=act_max) -> k-bit quantize (hardware_model.py:133-173, min 0) -> NHWC bf16
- * code pack for the next tcgen05 contraction.  fc stage (noisynet.py:540-569): the same with pool = 0,
+ * code pack for the next tensor-core contraction.  fc stage (noisynet.py:540-569): the same with pool = 0,
  * H = W = 1.  Per-channel reductions use fixed-order partial sums (deterministic). */
 typedef struct nn_stage_args {
     const float* in;          /* [B,C,H,W] fp32 NCHW: the (noisy) conv / linear output               */
@@ -337,7 +337,7 @@ int nn_stage_fwd(const nn_stage_args* a, int device, void* stream);
 
 /* Backward of the stage: masks of the quantizer STE (hardware_model.py:176-183), clamp and ReLU, BatchNorm
  * backward (dgamma / dbeta are OVERWRITTEN), max-pool routing; emits the gradient w.r.t. the stage input as
- * NHWC bf16 [B,H,W,Cp] -- the operand the tcgen05 wgrad / dgrad kernels read -- and optionally NCHW fp32. */
+ * NHWC bf16 [B,H,W,Cp] -- the operand the tensor-core wgrad / dgrad kernels read -- and optionally NCHW fp32. */
 typedef struct nn_stage_bwd_args {
     const float* g;           /* grad w.r.t. the stage output, NCHW fp32 (pooled shape)               */
     const float* x;           /* the BN input saved by the forward (pooled if pool = 1, else `in`)    */

@@ -1,4 +1,4 @@
-"""noisynet_b200 -- B200 (sm_100a) implementation of NoisyNet's quantized-conv + analog-noise hot path.
+"""noisynet_b200 -- H100 (sm_90a) implementation of NoisyNet's quantized-conv + analog-noise hot path.
 
 Public surface (mirrors the reference's operator API, SURVEY.md section 8b):
     noisynet_b200.hardware_model : NoisyConv2d, NoisyLinear, QuantMeasure, UniformQuantize, AddNoise,

@@ -1,6 +1,6 @@
 // C-ABI entry points for the fused noisy conv / linear forward and its backward.
 // Validates arguments and dispatches on `precision` to the CUDA-core fp32 kernels
-// (nn_conv_simt.cu) or the tcgen05 kernels (nn_conv_umma.cu).  No CPU fallback exists.
+// (nn_conv_simt.cu) or the tensor-core kernels (nn_conv_umma.cu, nn_conv_tma.cu).  No CPU fallback exists.
 #include "nn_common.cuh"
 
 int nn_simt_conv_fwd(const nn_conv_fwd_args* a, int device, cudaStream_t st);
@@ -55,7 +55,7 @@ extern "C" int nn_noisy_conv_fwd(const nn_conv_fwd_args* a, int device, void* st
         return nn_fail("nn_noisy_conv_fwd: y missing%s", "");
     }
     if (a->pooled_out && a->precision == NN_PREC_FP32)
-        return nn_fail("nn_noisy_conv_fwd: pooled_out is a tcgen05-path fusion%s (see nn_conv_pool_fusable)", "");
+        return nn_fail("nn_noisy_conv_fwd: pooled_out is a tensor-core-path fusion%s (see nn_conv_pool_fusable)", "");
     NN_SET_DEVICE(device);
     if (a->precision == NN_PREC_FP32) return nn_simt_conv_fwd(a, device, (cudaStream_t)stream);
     if (a->precision == NN_PREC_TF32)
@@ -63,7 +63,7 @@ extern "C" int nn_noisy_conv_fwd(const nn_conv_fwd_args* a, int device, void* st
                        "fp32 accumulate, 1.5e-2 tolerance) or NN_PREC_FP32", "");
     if (a->precision == NN_PREC_BF16) {
         if (!nn_umma_supports(&a->g, 0))
-            return nn_fail("nn_noisy_conv_fwd: geometry not supported by the tcgen05 path%s; use NN_PREC_FP32", "");
+            return nn_fail("nn_noisy_conv_fwd: geometry not supported by the tensor-core path%s; use NN_PREC_FP32", "");
         return nn_umma_conv_fwd(a, device, (cudaStream_t)stream);
     }
     return nn_fail("nn_noisy_conv_fwd: unknown precision%s", "");
@@ -79,7 +79,7 @@ extern "C" int nn_noisy_conv_dgrad(const nn_conv_dgrad_args* a, int device, void
     if (a->precision == NN_PREC_FP32) return nn_simt_conv_dgrad(a, device, (cudaStream_t)stream);
     if (a->precision != NN_PREC_BF16) return nn_fail("nn_noisy_conv_dgrad: precision not implemented%s (NN_PREC_FP32 / NN_PREC_BF16)", "");
     if (!nn_umma_supports(&a->g, 1))
-        return nn_fail("nn_noisy_conv_dgrad: geometry not supported by the tcgen05 path%s; use NN_PREC_FP32", "");
+        return nn_fail("nn_noisy_conv_dgrad: geometry not supported by the tensor-core path%s; use NN_PREC_FP32", "");
     return nn_umma_conv_dgrad(a, device, (cudaStream_t)stream);
 }
 
@@ -98,6 +98,6 @@ extern "C" int nn_noisy_conv_wgrad(const nn_conv_wgrad_args* a, int device, void
     if (a->precision == NN_PREC_FP32) return nn_simt_conv_wgrad(a, device, (cudaStream_t)stream);
     if (a->precision != NN_PREC_BF16) return nn_fail("nn_noisy_conv_wgrad: precision not implemented%s (NN_PREC_FP32 / NN_PREC_BF16)", "");
     if (!nn_umma_supports(&a->g, 2))
-        return nn_fail("nn_noisy_conv_wgrad: geometry not supported by the tcgen05 path%s; use NN_PREC_FP32", "");
+        return nn_fail("nn_noisy_conv_wgrad: geometry not supported by the tensor-core path%s; use NN_PREC_FP32", "");
     return nn_umma_conv_wgrad(a, device, (cudaStream_t)stream);
 }

@@ -98,7 +98,7 @@ k_allreduce_twoshot(const ArP p) {
     const long long per = p.n_vec / p.world, v0 = (long long)p.rank * per;
     if (p.mc_base) {
         // four independent switch round trips in flight per thread: the loop is bound by the ld_reduce latency (~2-3 us), not
-        // by bandwidth (measured at 2 ranks: one vector per iteration 103 us for 5.5 MB, NCCL 43 us)
+        // by bandwidth
         char* mc = reinterpret_cast<char*>(p.mc_base) + p.data_off + v0 * 16;
         const long long stride = (long long)gridDim.x * blockDim.x;
         long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;

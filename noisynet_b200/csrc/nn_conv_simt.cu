@@ -1,6 +1,6 @@
 // CUDA-core fp32 implicit-GEMM kernels (NN_PREC_FP32): the reference-arithmetic path.
 // Any stride / padding; conv and linear (H=W=KH=KW=1).  These kernels define the exact-fp32
-// behaviour the tcgen05 kernels (nn_conv_umma.cu) are checked against on the device, and
+// behaviour the tensor-core kernels (nn_conv_umma.cu) are checked against on the device, and
 // serve geometries the tensor-core path does not take.
 //
 //  forward : M = B*OH*OW, N = Cout, K = Cin*KH*KW.  Two (three) accumulators per output:
@@ -339,7 +339,7 @@ k_conv_wgrad_simt(const WgP p) {
 
 }  // namespace
 
-// Shared with the tcgen05 path: sums split partials in a fixed order and applies the STE mask.
+// Shared with the tensor-core path: sums split partials in a fixed order and applies the STE mask.
 __global__ void __launch_bounds__(256)
 k_wgrad_reduce(const float* __restrict__ partial, int splits, int64_t n, float* __restrict__ gw,
                const float* __restrict__ w_raw, float lo, float hi) {

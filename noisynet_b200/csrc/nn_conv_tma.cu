@@ -1,5 +1,5 @@
-// Persistent implicit-GEMM conv on CTA pairs with TMA-staged operands (sm_100a): the tiled noisy-conv forward and
-// the dgrad of the layers whose im2col rows cannot be read in place (conv2 of NoisyNet, the ResNet 3x3 layers).
+// Persistent implicit-GEMM conv with TMA-staged operands (sm_90a): the tiled noisy-conv forward and the dgrad of the
+// layers whose im2col rows cannot be read in place (conv2 of NoisyNet, the ResNet 3x3 layers).
 //
 //   D[m, n] = sum_{tap, c} X[pixel(m) + tap, c] * Wp[n, tap, c]      m = output pixel, n = accumulator column
 //
@@ -8,25 +8,21 @@
 //   narrower box (16 / 32 channels -> SWIZZLE_32B / 64B tile, its own descriptor kind) instead of padding every tap to
 //   a multiple of 64 channels (65 channels -> K = 80 per tap, not 128).  Padding taps and tile rows past the tensor are
 //   zero-filled by the TMA unit: no thread computes an address.
-// * B operand: pre-swizzled weight image [n-tile][tap][group][cta rank], one cp.async.bulk per stage and CTA.
-// * CTA pair (cluster of 2, tcgen05 cta_group::2): one M = 256 MMA per K = 16 step covers both CTAs' 128 pixels; each CTA
-//   stages only HALF of the weight rows, which halves the L2 -> SM weight stream that bounded the one-CTA kernel.
-// * Persistent: a cluster walks (pixel-tile pair, n-tile) items; accumulators are double-buffered in TMEM (2 x 256
-//   columns), so the epilogue warps (tcgen05.ld -> scale, Philox / Box-Muller current noise -> NCHW stores) of item i
-//   overlap the MMAs of item i + 1.
-// * Warp roles: warps 1..P producers (one elected thread each; a thread owns whole stages round-robin: a tensor-map
-//   copy costs its issuing thread ~800 cycles, tools/microbench/tma_probe.cu), warp 0 MMA issuer (leader CTA; both CTAs'
-//   copies complete on the leader's barrier), warp P+1 TMEM allocator, 8 epilogue warps.
+// * B operand: pre-swizzled weight image [n-tile][tap][group][half][chunk rows]; per stage and chunk two tiled
+//   tensor-map copies (the two row halves) land the chunk's n_mma rows contiguously.
+// * Persistent: a CTA walks (128-pixel tile, n-tile) items.  Two MMA warpgroups (64 pixels each) accumulate the main
+//   and sigma^2 columns in registers and run the epilogue (scale, Philox / Box-Muller current noise -> NCHW stores)
+//   straight from the wgmma fragments, while the producers already fill the ring with the next item's operands.
+// * Warp roles: warps 0-7 the two MMA / epilogue warpgroups, warps 8 .. 8 + P - 1 producers (one elected thread each; a
+//   thread owns whole stages round-robin, since a tensor-map copy keeps its issuing thread busy for hundreds of cycles).
 #include "nn_conv_tma.h"
 
 #include <cuda.h>
 
-#include "nn_tcgen05.cuh"
+#include "nn_wgmma.cuh"
 
 namespace {
 
-constexpr int TC_MAX_EPI_WARPS = 16;    // epilogue warps per CTA: 8 or 16 (4 or 8 column slices per TMEM lane quarter)
-constexpr int TC_ACC_STRIDE = 256;       // TMEM columns between the two accumulator buffers
 constexpr int TC_MAX_STAGES = 8;
 
 struct TmaConvP {
@@ -34,58 +30,37 @@ struct TmaConvP {
     CUtensorMap mapb64, mapb_tail;       // weight image as rows of 128 B / of the tail width: boxes of n_half rows
     int M, OH, OW, Cout, stride, pad, KW, taps;
     int n_c64, tail_w, nc, gpt, n_groups;
-    int n_t, n_mma, n_half, n_tiles, main_col, sig_col;
-    int items, stages, a_stage, b_stage, n_prod, n_epi, tap_bytes;
+    int n_t, n_mma, n_half, n_tiles;
+    int items, stages, a_stage, b_stage, n_prod, tap_bytes;
     float y_scale, s_scale;
     float *y, *y_noisy;
-    int noise_mode;
     float current;
     const float* scale_dev;
     const float* z_inject;               // EPI 3: N(0,1) draws of the caller (parity hook), [B, Cout, OH, OW]
     nn_rng rng;
     int* err_flag;
-    long long* prof;                     // NN_KDEBUG builds: [cta][16] cycle counters of the roles (nn_debug_tma_profile)
-    int dbg_mode;                        // NN_KDEBUG builds: experiment switches (nn_debug_tma_mode): 1 no epilogue work,
-                                         // 2 operands loaded for the first ring revolution only, 4 no per-group clock reads
 };
-
-#ifdef NN_KDEBUG
-#define TC_T(var) const long long var = (p.dbg_mode & 4) ? 0ll : clock64()
-#define TC_ACC(slot, t0) do { if (!(p.dbg_mode & 4)) prof_acc[slot] += clock64() - (t0); } while (0)
-#else
-#define TC_T(var)
-#define TC_ACC(slot, t0)
-#endif
 
 // EPI 1: noisy (main + sigma accumulators, Philox z), EPI 2: plain, EPI 3: noisy with injected z (parity tests)
 template <int EPI>
-__global__ void __launch_bounds__((4 + 2 + TC_MAX_EPI_WARPS) * 32, 1)
+__global__ void __launch_bounds__((8 + 2) * 32, 1)
 k_conv_tma(const __grid_constant__ TmaConvP p) {
+    constexpr int MCH = EPI == 2 ? 4 : 2;        // 64-column register chunks of the main / sigma accumulators
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const int S = p.stages;
     const uint32_t stage_bytes = (uint32_t)(p.a_stage + p.b_stage);
     const uint32_t bar_base = base + (uint32_t)S * stage_bytes;
     const uint32_t full_bar = bar_base, empty_bar = bar_base + 8u * TC_MAX_STAGES;
-    const uint32_t accf_bar = bar_base + 24u * TC_MAX_STAGES, acce_bar = accf_bar + 16u, tmem_slot = acce_bar + 16u;
-    uint8_t* gen0 = smem_raw + (base - smem_u32(smem_raw));
-    volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(gen0 + (tmem_slot - base));
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);          // warp-uniform for the compiler: role branches are convergent
-    const uint32_t rank = cluster_ctarank();
-    const int cl = (int)(blockIdx.x >> 1), ncl = (int)(gridDim.x >> 1);
     const int P = p.n_prod;
 
     if (tid == 0) {
         for (int s = 0; s < S; ++s) {
-            mbar_init(full_bar + 8 * s, 1);          // leader only: its producer's arrive.expect_tx for BOTH CTAs' boxes
-            mbar_init(empty_bar + 8 * s, 1);         // the leader's tcgen05.commit (multicast to both CTAs)
-        }
-        mbar_init(empty_bar + 8 * (TC_MAX_STAGES - 1), 1);     // (kdebug experiments: a barrier nobody waits on)
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(accf_bar + 8 * b, 1);                     // leader's commit: accumulator buffer b complete (both CTAs)
-            mbar_init(acce_bar + 8 * b, 2 * (uint32_t)p.n_epi);      // leader only: both CTAs' epilogue warps have drained buffer b
+            mbar_init(full_bar + 8 * s, 1);          // the producer's arrive.expect_tx
+            mbar_init(empty_bar + 8 * s, 2);         // both MMA warpgroups have read the stage
         }
         fence_mbar_init();
         tma_prefetch_desc(&p.map64);
@@ -94,288 +69,164 @@ k_conv_tma(const __grid_constant__ TmaConvP p) {
         tma_prefetch_desc(&p.mapb_tail);
     }
     __syncthreads();
-    cluster_sync_all();                 // both CTAs' barriers exist before the paired allocation / any remote arrive
-    if (warp == P + 1) tmem_alloc_2cta(tmem_slot, 512);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot_g, 0);
     const int ohw = p.OH * p.OW;
 
-    // Role -> warp: the MMA issuer is WARP 0, the oldest warp of its scheduler -- the warp schedulers favour older warps,
-    // and an issuer that sits behind polling warps loses a third of the tensor pipe to issue gaps (measured: the same
-    // instruction stream runs at 607 cycles per stage from warp 0 and at 915 from warp 4 behind a polling warp 0).
-    if (warp >= 1 && warp <= P) {
-        // ---------------------------------------------------------------- producers (warps 1..P)
-        const int pw = warp - 1;
-#ifdef NN_KDEBUG
-        if (!(p.dbg_mode & 8)) {
-#else
-        {
-#endif
-#ifdef NN_KDEBUG
-            long long prof_acc[4] = {0, 0, 0, 0};
-            const long long t_begin = clock64();
-#endif
-            int s = 0, turn = 0;                                 // ring stage and producer turn of the current group (no div / mod)
-            uint32_t eph = 1u;                                   // parity to wait for on the stage's empty barrier
-            // (no function call inside the role loops: uniform registers do not survive calls, and a call to the watchdog
-            //  handler in the loop body forces every descriptor through R2UR on each use -- the loops break out instead)
-            int fail = 0;
-            for (int it = cl; it < p.items && !fail; it += ncl) {
-                const int pi = it / p.n_tiles, nt = it - pi * p.n_tiles;
-                const int m0 = (2 * pi + (int)rank) * 128;
-                const int b0 = m0 / ohw, r0 = m0 - b0 * ohw, oh0 = r0 / p.OW, ow0 = r0 - oh0 * p.OW;
-                const int iw0 = ow0 * p.stride - p.pad, ih0 = oh0 * p.stride - p.pad;
-                const long long wt = (long long)nt * p.taps * p.tap_bytes;           // byte offset of this n-tile's weight image
-                int kh = 0, kw = 0, gi = 0;
-                for (int g = 0; g < p.n_groups; ++g) {
-                    if (turn == pw) {
-                        TC_T(t0);
-                        if (!mbar_wait_backoff(empty_bar + 8 * s, eph)) { fail = 401; break; }
-                        TC_ACC(0, t0);
-                        TC_T(t1);
-                        const int ca = 2 * gi, cb = 2 * gi + 1;
-                        const int wa = ca < p.n_c64 ? 64 : p.tail_w;
-                        const int wb = cb < p.nc ? (cb < p.n_c64 ? 64 : p.tail_w) : 0;
-                        const uint32_t b_bytes = (uint32_t)(p.n_half * 2 * (wa + wb));
-                        const uint32_t a_dst = base + (uint32_t)s * stage_bytes, b_dst = a_dst + (uint32_t)p.a_stage;
-                        const uint32_t bar = full_bar + 8 * s;
-                        // the leader announces both CTAs' bytes; every copy of the pair completes on the leader's barrier
-#ifdef NN_KDEBUG
-                        if ((p.dbg_mode & 2) && (it != cl || g >= S)) {        // experiment: stale operands, no copies
-                            if (rank == 0 && elect_one_sync()) mbar_arrive(bar);
-                            __syncwarp();
-                            if (++gi == p.gpt) { gi = 0; if (++kw == p.KW) { kw = 0; ++kh; } }
-                            if (++turn == P) turn = 0;
-                            if (++s == S) { s = 0; eph ^= 1u; }
-                            continue;
-                        }
-#endif
-                        if (elect_one_sync()) {
-                        // the leader announces both CTAs' bytes; every copy of the pair completes on the leader's barrier
-                        if (rank == 0) mbar_arrive_expect_tx(bar, 2u * ((uint32_t)(256 * (wa + wb)) + b_bytes));
-                        tma_im2col_4d_2cta(a_dst, ca < p.n_c64 ? &p.map64 : &p.map_tail, bar, 64 * ca, iw0, ih0, b0, (uint16_t)kw, (uint16_t)kh);
-                        if (wb) tma_im2col_4d_2cta(a_dst + 256u * (uint32_t)wa, cb < p.n_c64 ? &p.map64 : &p.map_tail, bar, 64 * cb, iw0, ih0, b0,
-                                                   (uint16_t)kw, (uint16_t)kh);
-                        const int tap = kh * p.KW + kw;
-                        const long long boff = wt + (long long)tap * p.tap_bytes + (long long)gi * (p.n_half * 512) + (long long)rank * b_bytes;
-                        if (wa == 64) tma_tile_2d_2cta(b_dst, &p.mapb64, bar, 0, (int)(boff >> 7));
-                        else tma_tile_2d_2cta(b_dst, &p.mapb_tail, bar, 0, (int)(boff / (2 * wa)));
-                        if (wb) {
-                            const long long boff2 = boff + (long long)p.n_half * 2 * wa;
-                            if (wb == 64) tma_tile_2d_2cta(b_dst + (uint32_t)(p.n_half * 2 * wa), &p.mapb64, bar, 0, (int)(boff2 >> 7));
-                            else tma_tile_2d_2cta(b_dst + (uint32_t)(p.n_half * 2 * wa), &p.mapb_tail, bar, 0, (int)(boff2 / (2 * wb)));
-                        }
-                        }
-                        __syncwarp();
-                        TC_ACC(1, t1);
-                    }
-                    if (++gi == p.gpt) { gi = 0; if (++kw == p.KW) { kw = 0; ++kh; } }
-                    if (++turn == P) turn = 0;
-                    if (++s == S) { s = 0; eph ^= 1u; }
-                }
-            }
-            if (fail) nn_pipeline_abort(p.err_flag, fail);
-#ifdef NN_KDEBUG
-            if (p.prof && pw == 0 && lane == 0) {      // producer 0: [0] waiting for a free stage, [1] issuing copies, [2] total
-                long long* o = p.prof + (size_t)blockIdx.x * 16;
-                o[0] = prof_acc[0]; o[1] = prof_acc[1]; o[2] = clock64() - t_begin;
-            }
-#endif
-        }
-        __syncwarp();
-    } else if (warp == 0) {
-        // ---------------------------------------------------------------- MMA issuer (leader CTA only)
-        if (rank == 0) {
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.n_mma >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-            // descriptor templates of the two chunk kinds (64 channels: 128-byte rows; tail: tail_w * 2-byte rows): only the
-            // 14-bit start address changes from stage to stage -- the issue loop does integer adds, nothing else
-            const uint64_t d64 = umma_desc_kmajor(0u, 128u), dtl = umma_desc_kmajor(0u, p.tail_w ? 2u * (uint32_t)p.tail_w : 128u);
-            const int kt = p.tail_w >> 4;
-            int s = 0, li = 0, fail = 0;
-            uint32_t fph = 0u;                                   // parity to wait for on the stage's full barrier
-#ifdef NN_KDEBUG
-            long long prof_acc[4] = {0, 0, 0, 0};
-            const long long t_begin = clock64();
-#endif
-            for (int it = cl; it < p.items && !fail; it += ncl, ++li) {
-                const int buf = li & 1;
-                TC_T(ta);
-#ifdef NN_KDEBUG
-                if (!(p.dbg_mode & 16))
-#endif
-                if (!mbar_wait_cluster(acce_bar + 8 * buf, (((uint32_t)(li >> 1)) & 1u) ^ 1u)) { fail = 402; break; }
-                TC_ACC(0, ta);
-                tc_fence_after();
-                const uint32_t d = tmem_base + (uint32_t)(buf * TC_ACC_STRIDE);
-                int gi = 0;
-                for (int g = 0; g < p.n_groups; ++g) {
-                    TC_T(tf);
-#ifdef NN_KDEBUG
-                    if (!(p.dbg_mode & 8))
-#endif
-                    if (!mbar_wait(full_bar + 8 * s, fph)) { fail = 403; break; }
-                    TC_ACC(1, tf);
-                    TC_T(ti);
-                    // no tcgen05.fence::after_thread_sync here: the stage was written by TMA (async proxy, completion through the
-                    // mbarrier), not by tcgen05 operations of other threads -- and the fence makes the issuing thread wait until
-                    // the previous group's MMAs have DRAINED (measured: 1250 -> see profiles/r2_*), a bubble per stage
+    if (warp >= 8 && warp < 8 + P) {
+        // ---------------------------------------------------------------- producers
+        const int pw = warp - 8;
+        int s = 0, turn = 0;                                 // ring stage and producer turn of the current group (no div / mod)
+        uint32_t eph = 1u;                                   // parity to wait for on the stage's empty barrier
+        // (no function call inside the role loops: uniform registers do not survive calls -- the loops break out instead)
+        int fail = 0;
+        for (int it = blockIdx.x; it < p.items && !fail; it += gridDim.x) {
+            const int mt = it / p.n_tiles, nt = it - mt * p.n_tiles;
+            const int m0 = mt * 128;
+            const int b0 = m0 / ohw, r0 = m0 - b0 * ohw, oh0 = r0 / p.OW, ow0 = r0 - oh0 * p.OW;
+            const int iw0 = ow0 * p.stride - p.pad, ih0 = oh0 * p.stride - p.pad;
+            const long long wt = (long long)nt * p.taps * p.tap_bytes;           // byte offset of this n-tile's weight image
+            int kh = 0, kw = 0, gi = 0;
+            for (int g = 0; g < p.n_groups; ++g) {
+                if (turn == pw) {
+                    if (!mbar_wait_backoff(empty_bar + 8 * s, eph)) { fail = 401; break; }
                     const int ca = 2 * gi, cb = 2 * gi + 1;
-                    const bool a64 = ca < p.n_c64, has_b = cb < p.nc, b64 = cb < p.n_c64;
-                    const uint32_t a_s = (base + (uint32_t)s * stage_bytes) >> 4, b_s = a_s + ((uint32_t)p.a_stage >> 4);
+                    const int wa = ca < p.n_c64 ? 64 : p.tail_w;
+                    const int wb = cb < p.nc ? (cb < p.n_c64 ? 64 : p.tail_w) : 0;
+                    const uint32_t half_bytes = (uint32_t)(p.n_half * 2 * (wa + wb));      // one row half of the group's weights
+                    const uint32_t a_dst = base + (uint32_t)s * stage_bytes, b_dst = a_dst + (uint32_t)p.a_stage;
+                    const uint32_t bar = full_bar + 8 * s;
                     if (elect_one_sync()) {
-                    {
-                        const uint64_t ad = (a64 ? d64 : dtl) | (uint64_t)(a_s & 0x3FFFu), bd = (a64 ? d64 : dtl) | (uint64_t)(b_s & 0x3FFFu);
-                        const int ks = a64 ? 4 : kt;
-                        umma_bf16_2cta(d, ad, bd, idesc, g != 0);
-                        for (int k = 1; k < ks; ++k) umma_bf16_2cta(d, ad + 2 * k, bd + 2 * k, idesc, 1u);
-                    }
-                    if (has_b) {
-                        const uint32_t wa = a64 ? 64u : (uint32_t)p.tail_w;
-                        const uint32_t a2 = a_s + 16u * wa, b2 = b_s + (((uint32_t)p.n_half * 2u * wa) >> 4);
-                        const uint64_t ad = (b64 ? d64 : dtl) | (uint64_t)(a2 & 0x3FFFu), bd = (b64 ? d64 : dtl) | (uint64_t)(b2 & 0x3FFFu);
-                        const int ks = b64 ? 4 : kt;
-                        for (int k = 0; k < ks; ++k) umma_bf16_2cta(d, ad + 2 * k, bd + 2 * k, idesc, 1u);
-                    }
-#ifdef NN_KDEBUG
-                    if (p.dbg_mode & 8) umma_commit_2cta_mc(empty_bar + 8 * (TC_MAX_STAGES - 1), 3);      // free-running issue experiment
-                    else
-#endif
-                    umma_commit_2cta_mc(empty_bar + 8 * s, 3);       // both CTAs may refill stage s when these MMAs retire
+                        mbar_arrive_expect_tx(bar, (uint32_t)(256 * (wa + wb)) + 2u * half_bytes);
+                        tma_im2col_4d(a_dst, ca < p.n_c64 ? &p.map64 : &p.map_tail, bar, 64 * ca, iw0, ih0, b0, (uint16_t)kw, (uint16_t)kh);
+                        if (wb) tma_im2col_4d(a_dst + 256u * (uint32_t)wa, cb < p.n_c64 ? &p.map64 : &p.map_tail, bar, 64 * cb, iw0, ih0, b0,
+                                              (uint16_t)kw, (uint16_t)kh);
+                        const int tap = kh * p.KW + kw;
+                        // chunk a of the group: rows [half 0 | half 1] at b_dst; chunk b after all n_mma rows of chunk a
+                        for (int h = 0; h < 2; ++h) {
+                            const long long boff = wt + (long long)tap * p.tap_bytes + (long long)gi * (p.n_half * 512) + (long long)h * half_bytes;
+                            const uint32_t da = b_dst + (uint32_t)(h * p.n_half * 2 * wa);
+                            if (wa == 64) tma_tile_2d(da, &p.mapb64, bar, 0, (int)(boff >> 7));
+                            else tma_tile_2d(da, &p.mapb_tail, bar, 0, (int)(boff / (2 * wa)));
+                            if (wb) {
+                                const long long boff2 = boff + (long long)p.n_half * 2 * wa;
+                                const uint32_t db = b_dst + (uint32_t)(p.n_mma * 2 * wa + h * p.n_half * 2 * wb);
+                                if (wb == 64) tma_tile_2d(db, &p.mapb64, bar, 0, (int)(boff2 >> 7));
+                                else tma_tile_2d(db, &p.mapb_tail, bar, 0, (int)(boff2 / (2 * wb)));
+                            }
+                        }
                     }
                     __syncwarp();
-                    TC_ACC(3, ti);
-#ifdef NN_KDEBUG
-                    if (p.prof && blockIdx.x == 0 && lane == 0 && !(p.dbg_mode & 4)) {      // per-group trace of cluster 0: stage ready / MMAs + commit issued
-                        const int tg = li * p.n_groups + g;
-                        if (tg < 1024) { p.prof[512 * 16 + 4 * tg] = tf; p.prof[512 * 16 + 4 * tg + 1] = ti; p.prof[512 * 16 + 4 * tg + 2] = clock64(); }
-                    }
-#endif
-                    if (++gi == p.gpt) gi = 0;
-                    if (++s == S) { s = 0; fph ^= 1u; }
                 }
-                if (!fail && elect_one_sync()) umma_commit_2cta_mc(accf_bar + 8 * buf, 3);          // both CTAs' accumulators of this item complete
-                __syncwarp();
+                if (++gi == p.gpt) { gi = 0; if (++kw == p.KW) { kw = 0; ++kh; } }
+                if (++turn == P) turn = 0;
+                if (++s == S) { s = 0; eph ^= 1u; }
             }
-            if (fail) nn_pipeline_abort(p.err_flag, fail);
-#ifdef NN_KDEBUG
-            if (p.prof && lane == 0) {     // MMA thread: waiting for [4] a drained accumulator, [5] the stage; [7] issuing; [8] total
-                long long* o = p.prof + (size_t)blockIdx.x * 16;
-                o[4] = prof_acc[0]; o[5] = prof_acc[1]; o[6] = prof_acc[2]; o[7] = prof_acc[3]; o[8] = clock64() - t_begin;
-            }
-#endif
         }
+        if (fail) nn_pipeline_abort(p.err_flag, fail);
         __syncwarp();
-    } else if (warp >= P + 2) {
-        // ---------------------------------------------------------------- epilogue warps
-        const int ew = warp - (P + 2);
-        const int q = warp & 3, slice = ew >> 2, nslices = p.n_epi >> 2;   // TMEM lane quarter = warp % 4; column slices round-robin
-        const bool noise = EPI != 2;
+    } else if (warp < 8) {
+        // ---------------------------------------------------------------- MMA warpgroups + epilogue
+        const int wg = warp >> 2, wt = tid & 127;
+        constexpr bool noise = EPI != 2;
         float coef = 0.f;
         NnRng rs = {0, 0, 0, 0};
         if (noise) { coef = nn_noise_coef(*p.scale_dev, p.current); rs = nn_rng_load(p.rng); }
         const int ngrp = (p.Cout + 3) >> 2;
-        const int nchunks = (p.n_t + 15) >> 4;
         const float y_scale = p.y_scale, s_scale = p.s_scale;
-        int li = 0;
-#ifdef NN_KDEBUG
-        long long prof_acc[4] = {0, 0, 0, 0};
-        const long long t_begin = clock64();
-        const int items_epi = (p.dbg_mode & 16) ? 0 : p.items;       // experiment: the MMA thread alone in the CTA
-#else
-        const int items_epi = p.items;
-#endif
-        int fail = 0;
-        for (int it = cl; it < items_epi; it += ncl, ++li) {
-            const int pi = it / p.n_tiles, nt = it - pi * p.n_tiles;
-            const int buf = li & 1;
-            TC_T(tw);
-            {   // one lane polls (256 threads hammering the barrier slow the MMA thread's own barrier traffic down)
-                int ok = 1;
-                if (lane == 0) ok = mbar_wait_backoff(accf_bar + 8 * buf, ((uint32_t)(li >> 1)) & 1u) ? 1 : 0;
-                ok = __shfl_sync(0xffffffffu, ok, 0);
-                if (!ok) { fail = 406; break; }
+        const int kt = p.tail_w >> 4;
+        int s = 0, fail = 0;
+        uint32_t fph = 0u;                                   // parity to wait for on the stage's full barrier
+        for (int it = blockIdx.x; it < p.items && !fail; it += gridDim.x) {
+            const int mt = it / p.n_tiles, nt = it - mt * p.n_tiles;
+            float accm[MCH][32], accs[2][32];
+            int gi = 0;
+            for (int g = 0; g < p.n_groups; ++g) {
+                if (!mbar_wait(full_bar + 8 * s, fph)) { fail = 403; break; }
+                const int ca = 2 * gi, cb = 2 * gi + 1;
+                const bool has_b = cb < p.nc;
+                const uint32_t a_s = base + (uint32_t)s * stage_bytes, b_s = a_s + (uint32_t)p.a_stage;
+                wg_fence();
+#pragma unroll 1
+                for (int ch = 0; ch < (has_b ? 2 : 1); ++ch) {
+                    const int w = (ch == 0 ? ca : cb) < p.n_c64 ? 64 : p.tail_w;      // channels of this chunk (row = 2 w bytes)
+                    const uint32_t a_c = a_s + (ch == 0 ? 0u : 256u * (uint32_t)(ca < p.n_c64 ? 64 : p.tail_w));
+                    const uint32_t b_c = b_s + (ch == 0 ? 0u : (uint32_t)(p.n_mma * 2 * (ca < p.n_c64 ? 64 : p.tail_w)));
+                    const uint64_t ad = gmma_desc_kmajor(a_c + (uint32_t)(wg * 64 * 2 * w), 2u * (uint32_t)w);
+                    const uint64_t bm = gmma_desc_kmajor(b_c, 2u * (uint32_t)w);
+                    const uint64_t bsg = gmma_desc_kmajor(b_c + (uint32_t)(p.n_t * 2 * w), 2u * (uint32_t)w);    // sigma rows follow the main rows
+                    const uint32_t step = 8u * (uint32_t)w;               // 64 rows of B in descriptor units
+                    const int ks = w == 64 ? 4 : kt;
+#pragma unroll 1
+                    for (int k = 0; k < ks; ++k) {
+                        const int acc_on = (g != 0 || ch != 0 || k != 0) ? 1 : 0;
+                        wg_mma<MCH, 0, 0>(accm, ad + 2 * k, bm + 2 * k, step, p.n_t, acc_on);
+                        if (noise) wg_mma<2, 0, 0>(accs, ad + 2 * k, bsg + 2 * k, step, p.n_t, acc_on);
+                    }
+                }
+                wg_commit();
+                wg_wait_all();
+                wg_fence_acc(accm);
+                if (noise) wg_fence_acc(accs);
+                __syncwarp();
+                if ((warp & 3) == 0 && elect_one_sync()) mbar_arrive(empty_bar + 8 * s);      // the stage may be refilled
+                __syncwarp();
+                if (++gi == p.gpt) gi = 0;
+                if (++s == S) { s = 0; fph ^= 1u; }
             }
-            TC_ACC(0, tw);
-            tc_fence_after();
-            const int row = q * 32 + lane;
-            const int m = (2 * pi + (int)rank) * 128 + row;
-            const bool row_ok = m < p.M;
-            int b = 0, pix = 0;
-            if (row_ok) { b = m / ohw; pix = m - b * ohw; }
-            const size_t out_row = (size_t)b * p.Cout * ohw + pix;
-            const uint32_t t_lane = tmem_base + (uint32_t)(buf * TC_ACC_STRIDE) + ((uint32_t)(q * 32) << 16);
+            if (fail) break;
+            // ---- epilogue from the fragments: rows r0, r0 + 8; columns 8 i + 2 (l % 4) + {0, 1} of each chunk.  The two
+            // lanes l, l ^ 1 share the 4-channel Philox groups of both rows: each draws one and hands over half of it.
+            const int r_top = 64 * wg + 16 * (wt >> 5) + (lane >> 2);
+            const int m_a = mt * 128 + r_top, m_b = m_a + 8;
+            const bool odd = (lane & 1) != 0;
+            const int m_own = odd ? m_b : m_a;
+            size_t orow[2];
+            bool ok[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int m = h ? m_b : m_a;
+                ok[h] = m < p.M;
+                const int b = ok[h] ? m / ohw : 0, pix = ok[h] ? m - b * ohw : 0;
+                orow[h] = (size_t)b * p.Cout * ohw + pix;
+            }
+            float* const out = EPI != 2 ? p.y_noisy : p.y;
             const int n_base = nt * p.n_t;
-            const uint64_t grp_row = (uint64_t)m * ngrp;
-            float* const out_main = (EPI != 2 ? p.y_noisy : p.y) + out_row;
-#ifdef NN_KDEBUG
-            if (p.dbg_mode & 1) goto epi_done;                        // experiment: accumulators dropped
-#endif
-            for (int ci = slice; ci < nchunks; ci += nslices) {
-                const int cc = ci * 16;
-                float am[16], as[16];
-                tmem_ld16(t_lane + (uint32_t)(p.main_col + cc), am);
-                if (EPI != 2) tmem_ld16(t_lane + (uint32_t)(p.sig_col + cc), as);
-                if (!row_ok) continue;
-                const int nb = n_base + cc;
-                const int nvalid = min(16, min(p.n_t - cc, p.Cout - nb));
-                float* o = out_main + (size_t)nb * ohw;
 #pragma unroll
-                for (int g4 = 0; g4 < 4; ++g4) {
-                    if (g4 * 4 < nvalid) {
-                        float z[4];
-                        if (EPI == 1) nn_normal4(rs, grp_row + (uint64_t)((nb + g4 * 4) >> 2), z);
-                        if (EPI == 3) {
+            for (int c = 0; c < MCH; ++c)
 #pragma unroll
-                            for (int j = 0; j < 4; ++j)
-                                z[j] = (g4 * 4 + j < nvalid) ? __ldg(p.z_inject + out_row + (size_t)(nb + g4 * 4 + j) * ohw) : 0.f;
-                        }
-                        if (g4 * 4 + 4 <= nvalid) {
-                            float* o_run = o + (size_t)(g4 * 4) * ohw;
-                            asm volatile("" : "+l"(o_run));
+                for (int i = 0; i < 8; ++i) {
+                    const int nl = 64 * c + 8 * i + 2 * (lane & 3);        // local column of register 4 i (+1: next column)
+                    if (64 * c + 8 * i >= p.n_t) continue;                 // warp-uniform
+                    const int n = n_base + nl;
+                    float z[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+                    if (EPI == 1) {
+                        float zz[4];
+                        nn_normal4(rs, (uint64_t)m_own * ngrp + (uint64_t)(n >> 2), zz);
+                        // even lane keeps z[0..1] of row a, gets z[0..1] of row b; odd lane keeps z[2..3] of row b, gets those of row a
+                        const float o0 = __shfl_xor_sync(0xffffffffu, odd ? zz[0] : zz[2], 1);
+                        const float o1 = __shfl_xor_sync(0xffffffffu, odd ? zz[1] : zz[3], 1);
+                        if (odd) { z[0][0] = o0; z[0][1] = o1; z[1][0] = zz[2]; z[1][1] = zz[3]; }
+                        else { z[0][0] = zz[0]; z[0][1] = zz[1]; z[1][0] = o0; z[1][1] = o1; }
+                    }
 #pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const int e = g4 * 4 + j;
-                                const float yv = am[e] * y_scale;
-                                st_global_f32(o_run, (EPI != 2) ? __fadd_rn(yv, __fmul_rn(z[j], nn_sigma(coef, as[e] * s_scale))) : yv);
-                                o_run += ohw;
-                            }
-                        } else {
+                    for (int h = 0; h < 2; ++h) {
+                        if (!ok[h]) continue;
 #pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const int e = g4 * 4 + j;
-                                if (e < nvalid) {
-                                    const float yv = am[e] * y_scale;
-                                    o[(size_t)e * ohw] = (EPI != 2) ? __fadd_rn(yv, __fmul_rn(z[j], nn_sigma(coef, as[e] * s_scale))) : yv;
-                                }
+                        for (int j = 0; j < 2; ++j) {
+                            if (nl + j >= p.n_t || n + j >= p.Cout) continue;
+                            const size_t o = orow[h] + (size_t)(n + j) * ohw;
+                            const float yv = accm[c][4 * i + 2 * h + j] * y_scale;
+                            if (EPI == 2) {
+                                out[o] = yv;
+                            } else {
+                                const float zv = EPI == 3 ? __ldg(p.z_inject + o) : z[h][j];
+                                out[o] = __fadd_rn(yv, __fmul_rn(zv, nn_sigma(coef, accs[c & 1][4 * i + 2 * h + j] * s_scale)));      // (MCH == 2)
                             }
                         }
                     }
                 }
-            }
-#ifdef NN_KDEBUG
-        epi_done:
-#endif
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {                                  // this warp has drained buffer `buf`: tell the leader's MMA thread
-                if (rank == 0) mbar_arrive(acce_bar + 8 * buf);
-                else mbar_arrive_remote(acce_bar + 8 * buf, 0);
-            }
         }
         if (fail) nn_pipeline_abort(p.err_flag, fail);
-#ifdef NN_KDEBUG
-        if (p.prof && ew == 0 && lane == 0) {   // first epilogue warp: [10] waiting for accumulators, [11] total, [12] items
-            long long* o = p.prof + (size_t)blockIdx.x * 16;
-            o[10] = prof_acc[0]; o[11] = clock64() - t_begin; o[12] = li;
-        }
-#endif
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                 // both CTAs are done with the paired accumulators / no remote arrive is in flight
-    if (warp == P + 1) { tc_fence_after(); tmem_dealloc_2cta(tmem_base, 512); }
 }
 
 typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const int*,
@@ -442,30 +293,8 @@ int encode_weight_map(CUtensorMap* map, const void* wp, size_t wp_bytes, int row
 }
 
 int g_tma_enable = 1;
-int g_tma_dbg_mode = 0;
-long long* g_prof_buf = nullptr;
-int g_prof_ctas = 0;
 
 }  // namespace
-
-extern "C" int nn_debug_tma_mode(int mode) { const int prev = g_tma_dbg_mode; if (mode >= 0) g_tma_dbg_mode = mode; return prev; }
-
-// NN_KDEBUG builds: per-CTA role cycle counters [cta][16] of the last k_conv_tma launch (tools/tma_profile.py)
-extern "C" int nn_debug_tma_trace(long long* host_out, int max_groups) {      // [group][4]: wait begin, stage ready, issued, -
-    if (!g_prof_buf) return 0;
-    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
-    const int n = max_groups < 1024 ? max_groups : 1024;
-    if (cudaMemcpy(host_out, g_prof_buf + 512 * 16, (size_t)n * 4 * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
-    return n;
-}
-
-extern "C" int nn_debug_tma_profile(long long* host_out, int max_ctas) {
-    if (!g_prof_buf) return 0;
-    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
-    const int n = g_prof_ctas < max_ctas ? g_prof_ctas : max_ctas;
-    if (cudaMemcpy(host_out, g_prof_buf, (size_t)n * 16 * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
-    return n;
-}
 
 extern "C" int nn_debug_tma_enable(int enable) {
     const int prev = g_tma_enable;
@@ -501,8 +330,7 @@ bool nn_tma_make_plan(int Cin_k, int KH, int KW, int stride, int pad, int n_out,
     if (pl.n_mma < 32) pl.n_mma = 32;
     if (pl.n_mma > 256) return false;
     pl.n_half = pl.n_mma / 2;
-    // the epilogue reads 16-column groups: every read must stay inside the 256-column buffer
-    if ((has_sigma ? pl.sig_col : pl.main_col) + tc_pad_to(pl.n_t, 16) > TC_ACC_STRIDE) return false;
+    if (pl.n_t > (has_sigma ? 128 : 256)) return false;     // register accumulators of the MMA warpgroups
     int gw = 0;                                     // widest group of a tap (channels)
     for (int gi = 0; gi < pl.gpt; ++gi) {
         const int ca = 2 * gi, cb = 2 * gi + 1;
@@ -510,16 +338,15 @@ bool nn_tma_make_plan(int Cin_k, int KH, int KW, int stride, int pad, int n_out,
         if (wa + wb > gw) gw = wa + wb;
     }
     pl.a_stage = tc_pad_to(256 * gw, 1024);
-    pl.b_stage = tc_pad_to(pl.n_half * 2 * gw, 1024);
+    pl.b_stage = tc_pad_to(pl.n_mma * 2 * gw, 1024);
     const int budget = 222 * 1024 - 2048;
     pl.stages = budget / (pl.a_stage + pl.b_stage);
-    if (pl.stages > TC_MAX_STAGES - 1) pl.stages = TC_MAX_STAGES - 1;      // (the last barrier slot serves the kdebug experiments)
+    if (pl.stages > TC_MAX_STAGES) pl.stages = TC_MAX_STAGES;
     if (pl.stages < 2) return false;
-    pl.n_prod = pl.stages < 4 ? pl.stages : 4;      // a producer may run at most one ring revolution ahead: n_prod <= stages
-    pl.n_epi = 8;          // measured: the epilogue warps wait for accumulators 80 % of the time; more warps only contend with the issue thread
-    pl.threads = (pl.n_prod + 2 + pl.n_epi) * 32;
+    pl.n_prod = 2;          // two producer warps (<= stages: a producer may run at most one ring revolution ahead)
+    pl.threads = (8 + pl.n_prod) * 32;
     pl.tap_bytes = 2 * pl.n_half * 2 * pl.wt;
-    pl.smem_bytes = 1024 + (size_t)pl.stages * (pl.a_stage + pl.b_stage) + 24 * TC_MAX_STAGES + 64;
+    pl.smem_bytes = 1024 + (size_t)pl.stages * (pl.a_stage + pl.b_stage) + 16 * TC_MAX_STAGES + 64;
     pl.wp_bytes = (size_t)pl.n_tiles * pl.taps * pl.tap_bytes;
     if (out) *out = pl;
     return true;
@@ -540,61 +367,22 @@ int nn_tma_conv_launch(const TmaConvCall& c, int device, cudaStream_t st) {
     if (pl.tail_w == 0) p.mapb_tail = p.mapb64;
     p.M = c.B * c.OH * c.OW; p.OH = c.OH; p.OW = c.OW; p.Cout = c.Cout; p.stride = c.stride; p.pad = c.pad; p.KW = c.KW; p.taps = pl.taps;
     p.n_c64 = pl.n_c64; p.tail_w = pl.tail_w; p.nc = pl.nc; p.gpt = pl.gpt; p.n_groups = pl.n_groups;
-    p.n_t = pl.n_t; p.n_mma = pl.n_mma; p.n_half = pl.n_half; p.n_tiles = pl.n_tiles; p.main_col = pl.main_col; p.sig_col = pl.sig_col;
-    const int m_tiles = (p.M + 127) / 128, m_pairs = (m_tiles + 1) / 2;
-    p.items = m_pairs * pl.n_tiles;
-    p.stages = pl.stages; p.a_stage = pl.a_stage; p.b_stage = pl.b_stage; p.n_prod = pl.n_prod; p.n_epi = pl.n_epi; p.tap_bytes = pl.tap_bytes;
-    p.y_scale = c.y_scale; p.s_scale = c.s_scale; p.y = c.y; p.y_noisy = c.y_noisy; p.noise_mode = c.noise_mode;
+    p.n_t = pl.n_t; p.n_mma = pl.n_mma; p.n_half = pl.n_half; p.n_tiles = pl.n_tiles;
+    p.items = ((p.M + 127) / 128) * pl.n_tiles;
+    p.stages = pl.stages; p.a_stage = pl.a_stage; p.b_stage = pl.b_stage; p.n_prod = pl.n_prod; p.tap_bytes = pl.tap_bytes;
+    p.y_scale = c.y_scale; p.s_scale = c.s_scale; p.y = c.y; p.y_noisy = c.y_noisy;
     p.current = c.current; p.scale_dev = c.scale_dev; p.z_inject = c.z_inject; p.rng = c.rng; p.err_flag = c.err_flag;
-    int clusters = nn_num_sms(device) / 2;
-    if (clusters > p.items) clusters = p.items;
-    if (clusters < 1) clusters = 1;
-#ifdef NN_KDEBUG
-    if (!g_prof_buf) cudaMalloc(&g_prof_buf, (512 * 16 + 4096) * sizeof(long long));
-    cudaMemsetAsync(g_prof_buf, 0, (512 * 16 + 4096) * sizeof(long long), st);
-    p.prof = g_prof_buf;
-    p.dbg_mode = g_tma_dbg_mode;
-    g_prof_ctas = 2 * clusters;
-#endif
+    int grid = nn_num_sms(device);          // persistent: one CTA per SM
+    if (grid > p.items) grid = p.items;
     NN_ONCE_PER_DEVICE({
         NN_CUDA_OK(cudaFuncSetAttribute(k_conv_tma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         NN_CUDA_OK(cudaFuncSetAttribute(k_conv_tma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         NN_CUDA_OK(cudaFuncSetAttribute(k_conv_tma<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     });
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(2 * clusters); cfg.blockDim = dim3(pl.threads); cfg.dynamicSmemBytes = pl.smem_bytes; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    {   // a persistent kernel must not launch more clusters than can be CO-RESIDENT: a CTA pair needs both SMs of one TPC,
-        // so GPCs with an odd number of enabled SMs leave one idle and fewer than SMs / 2 pairs fit -- a cluster that
-        // does not fit would only start after another one has walked ALL its items (a second wave of the whole kernel)
-        static int max_clusters[64][2] = {{0}};
-        static size_t for_smem[64][2] = {{0}};
-        const int ki = c.noise_mode != NN_NOISE_NONE ? 0 : 1;
-        if (device >= 0 && device < 64 && (!max_clusters[device][ki] || for_smem[device][ki] != pl.smem_bytes)) {
-            for_smem[device][ki] = pl.smem_bytes;
-            int n = 0;
-            cudaLaunchConfig_t q = cfg;
-            q.gridDim = dim3(2 * (nn_num_sms(device) / 2));
-            const cudaError_t e = ki == 0 ? cudaOccupancyMaxActiveClusters(&n, k_conv_tma<1>, &q) : cudaOccupancyMaxActiveClusters(&n, k_conv_tma<2>, &q);
-            max_clusters[device][ki] = (e == cudaSuccess && n > 0) ? n : nn_num_sms(device) / 2;
-            (void)cudaGetLastError();
-        }
-        if (device >= 0 && device < 64 && clusters > max_clusters[device][ki]) {
-            clusters = max_clusters[device][ki];
-            cfg.gridDim = dim3(2 * clusters);
-        }
-    }
-#ifdef NN_KDEBUG
-    g_prof_ctas = 2 * clusters;
-#endif
     if (c.ev0) cudaEventRecord((cudaEvent_t)c.ev0, st);          // measurement hook: brackets the kernel, not the host-side descriptor encoding
-    if (c.noise_mode != NN_NOISE_NONE && c.z_inject) NN_CUDA_OK(cudaLaunchKernelEx(&cfg, k_conv_tma<3>, p));
-    else if (c.noise_mode != NN_NOISE_NONE) NN_CUDA_OK(cudaLaunchKernelEx(&cfg, k_conv_tma<1>, p));
-    else NN_CUDA_OK(cudaLaunchKernelEx(&cfg, k_conv_tma<2>, p));
+    if (c.noise_mode != NN_NOISE_NONE && c.z_inject) k_conv_tma<3><<<grid, pl.threads, pl.smem_bytes, st>>>(p);
+    else if (c.noise_mode != NN_NOISE_NONE) k_conv_tma<1><<<grid, pl.threads, pl.smem_bytes, st>>>(p);
+    else k_conv_tma<2><<<grid, pl.threads, pl.smem_bytes, st>>>(p);
     if (c.ev1) cudaEventRecord((cudaEvent_t)c.ev1, st);
     NN_LAUNCH_OK();
     return 0;
@@ -622,8 +410,10 @@ int nn_tma_encode_rows(void* map_out, const void* ptr, uint64_t rows, uint64_t c
 // [64 reduction rows (pixels)][128 B = 64 channels] -- exactly what ONE tensor-map copy delivers: a tiled 2-D box of
 // grad_output (64 pixels x 64 output channels) and an im2col box of the layer input (64 pixels x 64 channels of one tap).
 // A CTA owns up to four (tap, 64-channel chunk) atoms = 256 accumulator columns and a share of the pixels; per 64-pixel
-// k-block six copies (48 KB) replace the 3072 cp.async gathers of the thread-gathered kernel.  Channel remainders of a
-// tap (Cp % 64 == 8, e.g. the 65 -> 72 channels of NoisyNet's conv2) stay on the gathered kernel (k_wgrad_umma, tail mode).
+// k-block six copies (48 KB) replace the 3072 cp.async gathers of the thread-gathered kernel.  An 8-channel remainder of
+// each tap (the 65 -> 72 channels of NoisyNet's conv2) is a second launch of the same kernel (TAIL): its B operand is a slab
+// of one {8 channels, 64 pixels} im2col copy per tap (SWIZZLE_NONE MN-major core matrices, taps 1 KB apart), 8 columns
+// per tap.  Two MMA warpgroups (64 output channels each) accumulate in registers and store the partial sums.
 namespace {
 
 struct WgTmaP {
@@ -631,74 +421,63 @@ struct WgTmaP {
     CUtensorMap map_x;               // im2col {Cp, W, H, B}, box {64 channels, 64 pixels}, SWIZZLE_128B
     CUtensorMap map_xt;              // im2col, box {8 channels, 64 pixels}, SWIZZLE_NONE: the channel remainder of a tap
     int OH, OW, stride, pad, KW, n_c64, n_atoms, Mpix, Cout;
-    int tiles_k, taps, tail_w;       // tail_w = 8: every tiles_k-th k-block also feeds the remainder accumulator
+    int taps;
     int num_kb, kb_per_split, stages, cols_pad;
     float* partial;                  // [splits][Cout][cols_pad]
-    float* partial_tail;             // [splits * tiles_k][Cout][256]: column tap * 8 + e <-> channel 64 * n_c64 + e
+    float* partial_tail;             // [splits][Cout][256]: column tap * 8 + e <-> channel 64 * n_c64 + e
     int* err_flag;
 };
 
-constexpr int WT_STAGE = 16384 + 32768;        // A: 2 atoms, B: 4 atoms of 8 KB
-constexpr int WT_TAIL = 32768;                 // the remainder slab: one [64 pixels][16 B] KB per tap, up to 32 taps
-constexpr int WT_PROD = 6;                     // producer warps (warp 0 MMA, 1..6 producers, 7 TMEM, 8..11 epilogue)
-constexpr int WT_THREADS = (2 + WT_PROD + 4) * 32;
+constexpr int WT_STAGE = 16384 + 32768;        // A: 2 atoms, B: 4 atoms of 8 KB (or the remainder slab: 1 KB per tap, <= 32 taps)
+constexpr int WT_PROD = 4;                     // producer warps (warps 0-7 MMA warpgroups, 8-11 producers)
+constexpr int WT_THREADS = (8 + WT_PROD) * 32;
 
+template <bool TAIL>
 __global__ void __launch_bounds__(WT_THREADS, 1)
 k_wgrad_tma(const __grid_constant__ WgTmaP p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const int S = p.stages;
-    const uint32_t tail_base = base + (uint32_t)S * WT_STAGE;
-    const uint32_t bar_base = tail_base + (p.tail_w ? (uint32_t)WT_TAIL : 0u);
-    const uint32_t full_bar = bar_base, empty_bar = bar_base + 64u, tfull_bar = bar_base + 128u;
-    const uint32_t rfull_bar = bar_base + 136u, rempty_bar = bar_base + 144u, tmem_slot = bar_base + 152u;   // r*: the remainder slab
-    uint8_t* gen0 = smem_raw + (base - smem_u32(smem_raw));
-    volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(gen0 + (tmem_slot - base));
+    const uint32_t bar_base = base + (uint32_t)S * WT_STAGE;
+    const uint32_t full_bar = bar_base, empty_bar = bar_base + 64u;
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
     const int tile_k = blockIdx.x, tile_n = blockIdx.y, split = blockIdx.z;
     const int kb0 = split * p.kb_per_split, kb1 = min(p.num_kb, kb0 + p.kb_per_split);
     const int nkb = max(0, kb1 - kb0);
-    const int atoms = min(4, p.n_atoms - tile_k * 4);           // (tap, chunk) atoms of this column tile
-    const int n_cols = 64 * atoms;
-    const int t_cols = (p.taps * 8 + 15) & ~15;                 // remainder accumulator: 8 columns per tap
-    const uint32_t tmem_cols = p.tail_w ? 512u : 256u;
-    // the remainder columns of k-block kb belong to the CTA with tile_k == kb % tiles_k (same split): the work is spread over
-    // all CTAs, and the k-block's grad_output operand is already in the stage
+    const int atoms = TAIL ? 0 : min(4, p.n_atoms - tile_k * 4);  // (tap, chunk) atoms of this column tile
+    const int n_cols = TAIL ? (p.taps * 8 + 15) & ~15 : 64 * atoms;
     if (tid == 0) {
-        for (int s = 0; s < S; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 1); }
-        mbar_init(tfull_bar, 1);
-        mbar_init(rfull_bar, 1);
-        mbar_init(rempty_bar, 1);
+        for (int s = 0; s < S; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 2); }
         fence_mbar_init();
         tma_prefetch_desc(&p.map_gy);
-        tma_prefetch_desc(&p.map_x);
-        if (p.tail_w) tma_prefetch_desc(&p.map_xt);
+        if (TAIL) tma_prefetch_desc(&p.map_xt);
+        else tma_prefetch_desc(&p.map_x);
     }
-    if (warp == WT_PROD + 1) tmem_alloc(tmem_slot, tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot_g, 0);
     int fail = 0;
 
-    if (warp >= 1 && warp <= WT_PROD) {
-        // ---- producers: one elected lane per warp issues its share of a stage's copies (an im2col copy of 8 KB occupies its
-        // issuing thread for ~800 cycles, so the six copies of a stage go out from six warps); warp 1 also posts the byte count.
-        const int pw = warp - 1;
+    if (warp >= 8) {
+        // ---- producers: one elected lane per warp issues its share of a stage's copies (an im2col copy occupies its issuing
+        // thread for hundreds of cycles, so the copies of a stage go out from several warps); warp 8 also posts the byte count.
+        const int pw = warp - 8;
         const int ohw = p.OH * p.OW;
         for (int i = 0; i < nkb; ++i) {
             const int s = i % S;
             if (!mbar_wait_backoff(empty_bar + 8 * s, (((uint32_t)(i / S)) & 1u) ^ 1u)) { fail = 501; break; }
             const int m0 = (kb0 + i) * 64;
             const int b0 = m0 / ohw, r0 = m0 - b0 * ohw, oh0 = r0 / p.OW, ow0 = r0 - oh0 * p.OW;
-            const int n_copy = 2 + atoms;
+            const int n_copy = 2 + (TAIL ? p.taps : atoms);
             if (elect_one_sync()) {
                 const uint32_t dst = base + (uint32_t)s * WT_STAGE, bar = full_bar + 8 * s;
-                if (pw == 0) mbar_arrive_expect_tx(bar, 16384u + 8192u * (uint32_t)atoms);
+                if (pw == 0) mbar_arrive_expect_tx(bar, 16384u + (TAIL ? 1024u * (uint32_t)p.taps : 8192u * (uint32_t)atoms));
                 for (int j = pw; j < n_copy; j += WT_PROD) {
                     if (j < 2) {
                         tma_tile_2d(dst + 8192u * (uint32_t)j, &p.map_gy, bar, tile_n * 128 + 64 * j, m0);
+                    } else if (TAIL) {
+                        const int tap = j - 2, kh = tap / p.KW, kw = tap - kh * p.KW;
+                        tma_im2col_4d(dst + 16384u + 1024u * (uint32_t)tap, &p.map_xt, bar, 64 * p.n_c64, ow0 * p.stride - p.pad,
+                                      oh0 * p.stride - p.pad, b0, (uint16_t)kw, (uint16_t)kh);
                     } else {
                         const int a = j - 2, ga = tile_k * 4 + a, tap = ga / p.n_c64, ch = ga - tap * p.n_c64;
                         const int kh = tap / p.KW, kw = tap - kh * p.KW;
@@ -709,111 +488,53 @@ k_wgrad_tma(const __grid_constant__ WgTmaP p) {
             }
             __syncwarp();
         }
-    } else if (warp > WT_PROD && p.tail_w && warp - (WT_PROD + 1) < p.taps) {
-        // ---- remainder producers (the TMEM and epilogue warps, idle during the main loop): one [64 pixels][16 B] slab per tap,
-        // SWIZZLE_NONE MN-major core matrices (8 pixels x 16 B), taps 1 KB apart.  A copy occupies its issuing thread for
-        // hundreds of cycles whatever its size, so the taps go out from five warps that issue nothing else.  The slab is a
-        // one-slot pipeline of its own (rfull / rempty), filled up to tiles_k k-blocks ahead of its use.
-        const int tw = warp - (WT_PROD + 1);
-        const int ohw = p.OH * p.OW;
-        int i = ((tile_k - kb0 % p.tiles_k) + p.tiles_k) % p.tiles_k;
-        for (uint32_t t = 0; i < nkb; i += p.tiles_k, ++t) {
-            if (!mbar_wait_backoff(rempty_bar, (t & 1u) ^ 1u)) { fail = 504; break; }
-            const int m0 = (kb0 + i) * 64;
-            const int b0 = m0 / ohw, r0 = m0 - b0 * ohw, oh0 = r0 / p.OW, ow0 = r0 - oh0 * p.OW;
-            if (elect_one_sync()) {
-                if (tw == 0) mbar_arrive_expect_tx(rfull_bar, 1024u * (uint32_t)p.taps);
-                for (int tap = tw; tap < p.taps; tap += 5) {
-                    const int kh = tap / p.KW, kw = tap - kh * p.KW;
-                    tma_im2col_4d(tail_base + 1024u * (uint32_t)tap, &p.map_xt, rfull_bar, 64 * p.n_c64, ow0 * p.stride - p.pad,
-                                  oh0 * p.stride - p.pad, b0, (uint16_t)kw, (uint16_t)kh);
-                }
-            }
-            __syncwarp();
-        }
-    } else if (warp == 0) {
-        // ---- MMA issuer: MN-major A and B (bits 15, 16), M = 128 output channels, N = 64 x atoms (+ the remainder columns)
-        const uint32_t idesc0 = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(128 >> 4) << 24);
-        const uint32_t idesc = idesc0 | ((uint32_t)(n_cols >> 3) << 17), idesc_t = idesc0 | ((uint32_t)(t_cols >> 3) << 17);
-        const uint64_t d0 = umma_desc_sw128(0u) | ((uint64_t)((64u * 128u) >> 4) << 16);        // LBO = atom stride = 8192 B
-        // remainder slab: LBO = 8-pixel groups 128 B apart, SBO = the taps' slabs 1 KB apart; 16 pixels = 256 B
-        const uint64_t bt = umma_desc_none(tail_base, 8u, 64u);
-        int s = 0, n_tail = 0;
+    } else {
+        // ---- MMA warpgroups: MN-major A and B; warpgroup g owns output channels 64 g .. 64 g + 63 (the second atom of A, + 8 KB).
+        // B: main -- SWIZZLE_128B atoms (LBO = atom stride 8192 B, 16 pixels = 2048 B); remainder slab -- LBO = 8-pixel groups
+        // 128 B apart, SBO = the taps' slabs 1 KB apart, 16 pixels = 256 B
+        const int wg = warp >> 2;
+        const uint64_t da = gmma_desc(0u, 8192u >> 4, 1024u >> 4, 1u);
+        const uint64_t db = TAIL ? gmma_desc(0u, 8u, 64u, 0u) : da;
+        const uint32_t b_step = 512u, k_step_b = TAIL ? 16u : 128u;
+        float acc[4][32];
+        int s = 0;
         uint32_t ph = 0u;
         for (int i = 0; i < nkb; ++i) {
             if (!mbar_wait(full_bar + 8 * s, ph)) { fail = 502; break; }
-            const uint32_t a_s = (base + (uint32_t)s * WT_STAGE) >> 4, b_s = a_s + (16384u >> 4);
-            const bool with_tail = p.tail_w && ((kb0 + i) % p.tiles_k) == tile_k;
-            if (with_tail && !mbar_wait(rfull_bar, (uint32_t)n_tail & 1u)) { fail = 505; break; }
-            if (elect_one_sync()) {
-                const uint64_t ad = d0 | (uint64_t)(a_s & 0x3FFFu), bd = d0 | (uint64_t)(b_s & 0x3FFFu);
-                umma_bf16(tmem_base, ad, bd, idesc, i != 0);
+            const uint32_t a_s = (base + (uint32_t)s * WT_STAGE + (uint32_t)wg * 8192u) >> 4, b_s = (base + (uint32_t)s * WT_STAGE + 16384u) >> 4;
+            const uint64_t ad = da | (uint64_t)(a_s & 0x3FFFu), bd = db | (uint64_t)(b_s & 0x3FFFu);
+            wg_fence();
 #pragma unroll
-                for (int k = 1; k < 4; ++k) umma_bf16(tmem_base, ad + 128 * k, bd + 128 * k, idesc, 1u);     // 16 pixels = 2048 B
-                if (with_tail) {
-                    umma_bf16(tmem_base + 256u, ad, bt, idesc_t, n_tail != 0);
-#pragma unroll
-                    for (int k = 1; k < 4; ++k) umma_bf16(tmem_base + 256u, ad + 128 * k, bt + 16 * k, idesc_t, 1u);
-                    umma_commit(rempty_bar);
-                }
-                umma_commit(empty_bar + 8 * s);
-            }
+            for (int k = 0; k < 4; ++k) wg_mma<4, 1, 1>(acc, ad + 128 * k, bd + k_step_b * k, b_step, n_cols, (i | k) != 0 ? 1 : 0);
+            wg_commit();
+            wg_wait_all();
+            wg_fence_acc(acc);
             __syncwarp();
-            if (with_tail) ++n_tail;
+            if ((warp & 3) == 0 && elect_one_sync()) mbar_arrive(empty_bar + 8 * s);
+            __syncwarp();
             if (++s == S) { s = 0; ph ^= 1u; }
         }
-        if (elect_one_sync()) umma_commit(tfull_bar);
-        __syncwarp();
+        if (!fail) {
+            // ---- epilogue: rows = output channels, columns = (atom, channel) [or (tap, remainder channel)]
+            const int wt = tid & 127;
+            const int n0 = tile_n * 128 + 64 * wg + 16 * (wt >> 5) + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int n = n0 + 8 * h;
+                if (n >= p.Cout) continue;
+                float* out = TAIL ? p.partial_tail + ((size_t)split * p.Cout + n) * 256 + c0
+                                  : p.partial + ((size_t)split * p.Cout + n) * p.cols_pad + (size_t)tile_k * 256 + c0;
+#pragma unroll
+                for (int c = 0; c < 4; ++c)
+#pragma unroll
+                    for (int j = 0; j < 8; ++j)
+                        if (64 * c + 8 * j < n_cols)
+                            *reinterpret_cast<float2*>(out + 64 * c + 8 * j) =
+                                nkb > 0 ? make_float2(acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]) : make_float2(0.f, 0.f);
+            }
+        }
     }
     if (fail) nn_pipeline_abort(p.err_flag, fail);
-    if (warp >= WT_PROD + 2) {
-        // ---- epilogue: accumulator rows = output channels, columns = (atom, channel): partial[split][n][tile_k * 256 + col]
-        bool ok = true;
-        if (lane == 0) ok = mbar_wait_backoff(tfull_bar, 0);
-        ok = __shfl_sync(0xffffffffu, ok ? 1 : 0, 0) != 0;
-        if (!ok) nn_pipeline_abort(p.err_flag, 503);
-        tc_fence_after();
-        const int q = warp & 3;
-        const int n = tile_n * 128 + q * 32 + lane;
-        const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-        const int nrow = n < p.Cout ? n : 0;
-        float* out = p.partial + ((size_t)split * p.Cout + nrow) * p.cols_pad + (size_t)tile_k * 256;
-        for (int ci = 0; ci < (n_cols >> 4); ++ci) {
-            float v[16];
-            if (nkb > 0) tmem_ld16(t_lane + (uint32_t)(ci * 16), v);
-            else {
-#pragma unroll
-                for (int e = 0; e < 16; ++e) v[e] = 0.f;
-            }
-            if (n < p.Cout) {
-                float4* o4 = reinterpret_cast<float4*>(out + ci * 16);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) o4[e] = make_float4(v[4 * e], v[4 * e + 1], v[4 * e + 2], v[4 * e + 3]);
-            }
-        }
-        if (p.tail_w) {
-            // k-blocks of [kb0, kb1) congruent to tile_k: did this CTA accumulate any?
-            const int first = kb0 + ((tile_k - kb0 % p.tiles_k) + p.tiles_k) % p.tiles_k;
-            const bool any = first < kb1;
-            float* outt = p.partial_tail + ((size_t)(split * p.tiles_k + tile_k) * p.Cout + nrow) * 256;
-            for (int ci = 0; ci < (t_cols >> 4); ++ci) {
-                float v[16];
-                if (any) tmem_ld16(t_lane + 256u + (uint32_t)(ci * 16), v);
-                else {
-#pragma unroll
-                    for (int e = 0; e < 16; ++e) v[e] = 0.f;
-                }
-                if (n < p.Cout) {
-                    float4* o4 = reinterpret_cast<float4*>(outt + ci * 16);
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) o4[e] = make_float4(v[4 * e], v[4 * e + 1], v[4 * e + 2], v[4 * e + 3]);
-                }
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == WT_PROD + 1) { tc_fence_after(); tmem_dealloc(tmem_base, tmem_cols); }
 }
 
 }  // namespace
@@ -831,8 +552,6 @@ bool nn_tma_wgrad_plan(int Cin, int KH, int KW, int stride, int pad, int Cout, i
     // (zero-filled) 64-channel chunk
     if (w.tail_w > 8 || (w.tail_w == 8 && KH * KW > 31)) { w.n_c64 += 1; w.tail_w = 0; }
     w.stages = 4;
-    // (with fewer than four column tiles the one-slot remainder pipeline would be refilled every few k-blocks and stall)
-    if (w.tail_w && (KH * KW * w.n_c64 + 3) / 4 < 4) { w.n_c64 += 1; w.tail_w = 0; }
     w.Coutp = tc_pad_to(Cout, 8);
     w.taps = KH * KW;
     w.n_atoms = w.taps * w.n_c64;
@@ -846,9 +565,9 @@ bool nn_tma_wgrad_plan(int Cin, int KH, int KW, int stride, int pad, int Cout, i
     if (splits < 1) splits = 1;
     w.kb_per_split = (w.num_kb + splits - 1) / splits;
     w.splits = (w.num_kb + w.kb_per_split - 1) / w.kb_per_split;
-    w.smem_bytes = 1024 + (size_t)w.stages * WT_STAGE + (w.tail_w ? WT_TAIL : 0) + 256;
+    w.smem_bytes = 1024 + (size_t)w.stages * WT_STAGE + 256;
     w.main_bytes = ((size_t)w.splits * Cout * w.cols_pad * 4 + 1023) / 1024 * 1024;
-    w.partial_bytes = w.main_bytes + (w.tail_w ? (size_t)w.splits * w.tiles_k * Cout * 256 * 4 : 0);
+    w.partial_bytes = w.main_bytes + (w.tail_w ? (size_t)w.splits * Cout * 256 * 4 : 0);
     if (out) *out = w;
     return true;
 }
@@ -894,16 +613,20 @@ int nn_tma_wgrad_launch(const TmaWgradCall& c, int device, cudaStream_t st) {
             if (drv <= 13010 && (size_t)c.B * c.H * c.W * Cp * 2 < 131072) reinterpret_cast<uint64_t*>(&p.map_xt)[1] &= ~(1ull << 21);
         }
     }
-    p.tiles_k = w.tiles_k; p.taps = w.taps; p.tail_w = w.tail_w;
+    p.taps = w.taps;
     p.partial_tail = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c.partial) + w.main_bytes);
     p.OH = c.OH; p.OW = c.OW; p.stride = c.stride; p.pad = c.pad; p.KW = c.KW; p.n_c64 = w.n_c64; p.n_atoms = w.n_atoms;
     p.Mpix = c.B * c.OH * c.OW; p.Cout = c.Cout; p.num_kb = w.num_kb; p.kb_per_split = w.kb_per_split; p.stages = w.stages;
     p.cols_pad = w.cols_pad; p.partial = c.partial; p.err_flag = c.err_flag;
     NN_ONCE_PER_DEVICE({
-        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_tma, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_tma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     });
-    dim3 grid(w.tiles_k, w.m_tiles_n, w.splits);
-    k_wgrad_tma<<<grid, WT_THREADS, w.smem_bytes, st>>>(p);
+    k_wgrad_tma<false><<<dim3(w.tiles_k, w.m_tiles_n, w.splits), WT_THREADS, w.smem_bytes, st>>>(p);
     NN_LAUNCH_OK();
+    if (w.tail_w) {         // the 8-channel remainder columns of every tap: one column tile
+        k_wgrad_tma<true><<<dim3(1, w.m_tiles_n, w.splits), WT_THREADS, w.smem_bytes, st>>>(p);
+        NN_LAUNCH_OK();
+    }
     return 0;
 }

@@ -1,4 +1,4 @@
-// Persistent TMA-im2col implicit-GEMM conv kernel on CTA pairs (nn_conv_tma.cu): plan + launch interface used by the
+// Persistent TMA-im2col implicit-GEMM conv kernel (nn_conv_tma.cu): plan + launch interface used by the
 // entry points in nn_conv_umma.cu (forward: fused noisy conv; dgrad: forward over grad_output with flipped weights).
 #pragma once
 #include "nn_common.cuh"
@@ -7,9 +7,9 @@
 // 16 / 32 / 64 channels (SWIZZLE_32B / 64B / 128B); a pipeline stage ("group") holds up to two chunks of one tap.
 struct TmaPlan {
     int Cp, taps, n_c64, tail_w, wt, nc, gpt, n_groups;   // wt = padded channels per tap, nc = chunks per tap, gpt = groups per tap
-    int n_t, n_tiles, n_mma, n_half, main_col, sig_col;   // n-tiling as in the tiled kernels; n_half = rows staged per CTA of a pair
-    int stages, a_stage, b_stage, n_prod, n_epi, threads;
-    int tap_bytes;                                         // bytes of one tap of one n-tile in the weight image (both ranks)
+    int n_t, n_tiles, n_mma, n_half, main_col, sig_col;   // n-tiling as in the tiled kernels; n_half = rows of one weight-copy box
+    int stages, a_stage, b_stage, n_prod, threads;
+    int tap_bytes;                                         // bytes of one tap of one n-tile in the weight image (both halves)
     size_t smem_bytes, wp_bytes;
 };
 
@@ -38,7 +38,7 @@ int nn_tma_conv_launch(const TmaConvCall& c, int device, cudaStream_t st);
 
 // ---- weight gradient with TMA-staged operands (k_wgrad_tma): the (tap, 64-channel chunk) columns of the gradient
 struct TmaWgradPlan {
-    int Cp, Coutp, taps, n_c64, tail_w;        // tail_w: 0 or 8 channels per tap left to the gathered kernel
+    int Cp, Coutp, taps, n_c64, tail_w;        // tail_w: 0 or 8 channels per tap (the remainder launch)
     int n_atoms, tiles_k, cols_pad, m_tiles_n, num_kb, kb_per_split, splits, stages;
     size_t smem_bytes, main_bytes, partial_bytes;      // partial = [main | remainder accumulators]
 };

@@ -1,4 +1,4 @@
-// tcgen05 (5th-gen tensor core) implicit-GEMM kernels for the fused noisy conv / linear (sm_100a).
+// Warpgroup-MMA (wgmma, sm_90a) implicit-GEMM kernels for the fused noisy conv / linear.
 //
 //   D[m, n] = sum_k A[m, k] * B[n, k]        m = output pixel (b, oh, ow), k = (tap, c), n = output channel
 //
@@ -10,12 +10,12 @@
 // * B (weights) is packed once per call into the exact swizzled shared-memory image, one contiguous
 //   block per (n-tile, k-block), so a single cp.async.bulk (TMA engine, mbarrier complete_tx) stages it.
 //   Rows of a tile:  [ main weights n_t | g(|w_raw|) n_t | colsum(|w_raw|) 1 | zero pad ]  -> ONE
-//   tcgen05.mma per 16-wide k step feeds the Y, sigma^2 and power-statistic accumulators from one A tile.
-// * Accumulators live in TMEM (128 lanes x n_mma fp32 columns); the epilogue reads them with
-//   tcgen05.ld, applies scale/bias, draws Philox normals, adds sigma*z and writes NCHW fp32.
-// * Warp roles: warps 0-3 cp.async producers, warp 4 MMA issuer (one elected thread) + TMEM alloc,
-//   warp 5 weight bulk-copy issuer; all 8 warps run the epilogue.  2 CTAs/SM (<= 100 KB smem, 256 TMEM
-//   columns each) so one CTA's epilogue overlaps the other's main loop.
+//   MMA per 16-wide k step feeds the Y, sigma^2 and power-statistic accumulators from one A tile.
+// * Two consumer warpgroups (64 rows of the 128-row tile each) accumulate in registers; after the last k-block they
+//   write the accumulators to a shared-memory tile (over the then idle operand ring) and run the epilogue from it: scale /
+//   bias, Philox normals, sigma*z, NCHW fp32 stores.
+// * Warp roles: warps 0-3 cp.async producers (warp 0 also issues the weight bulk copy), warps 4-11 the two MMA
+//   warpgroups, which then run the epilogue.
 // * Every mbarrier wait is bounded (clock64 watchdog): a protocol bug sets an error flag instead of
 //   hanging the GPU.
 #include <cuda_bf16.h>
@@ -23,14 +23,15 @@
 #include <stdlib.h>
 
 #include "nn_common.cuh"
-#include "nn_tcgen05.cuh"
+#include "nn_wgmma.cuh"
 #include "nn_conv_tma.h"
 
 namespace {
 
 constexpr int UM_BLOCK_M = 128;
 constexpr int UM_BLOCK_K = 64;                       // bf16 per k-block = 128 bytes = one SWIZZLE_128B row
-constexpr int UM_THREADS = 256;
+constexpr int UM_THREADS = 384;                     // 4 producer warps + 2 MMA / epilogue warpgroups
+constexpr int UM_ACC_CH = 4;                         // 64-column accumulator chunks per warpgroup (up to 256 columns)
 constexpr int UM_A_STAGE = UM_BLOCK_M * 128;         // 16 KB
 constexpr int UM_MAX_NT = 120;                       // output channels per n-tile when sigma rows are present
 
@@ -38,8 +39,9 @@ constexpr int UM_MAX_NT = 120;                       // output channels per n-ti
 struct UmmaP {
     int B, H, W, Cp;               // packed input  [B, H, W, Cp] bf16
     int KH, KW, stride, pad, OH, OW;
-    int M, Cout, n_t, n_mma, num_kb, stages, tmem_cols;
+    int M, Cout, n_t, n_mma, num_kb, stages, acc_cols;
     int main_col, sig_col, wsum_col;   // accumulator column offsets inside an n-tile, -1 = absent
+    int ring_bytes;                    // max(operand ring, accumulator tile): the barriers follow
     const __nv_bfloat16* xp;
     const __nv_bfloat16* wp;       // [n_tiles][num_kb][n_mma * 64] bf16, pre-swizzled smem image
     float y_scale, s_scale;
@@ -73,11 +75,8 @@ struct UmmaAMap { alignas(64) unsigned char bytes[128]; };      // CUtensorMap o
 // y_noisy [+ y], no bias / mask / inject / export / stats) -- the training hot path, 2 = lean plain (y only).
 // The epilogue is issue-bound (Philox + Box-Muller per output), so the hot variants carry no per-element
 // option checks.
-#ifndef NN_EPI1_MINBLOCKS
-#define NN_EPI1_MINBLOCKS 2
-#endif
 template <int EPI>
-__global__ void __launch_bounds__(UM_THREADS, EPI == 2 ? 3 : (EPI == 1 ? NN_EPI1_MINBLOCKS : 2))
+__global__ void __launch_bounds__(UM_THREADS, 1)
 k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -85,14 +84,13 @@ k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
     const uint32_t b_stage = (uint32_t)p.n_mma * 128u;
     const uint32_t a_base = base;
     const uint32_t b_base = base + (uint32_t)S * UM_A_STAGE;
-    const uint32_t bar_base = b_base + (uint32_t)S * b_stage;      // 8-byte barriers: full[S], empty[S], tmem_full
-    const uint32_t full_bar = bar_base, empty_bar = bar_base + 8u * S, tfull_bar = bar_base + 16u * S;
-    const uint32_t tmem_slot = tfull_bar + 8;
-    const uint32_t abort_slot = tmem_slot + 4;
-    // generic pointers to the two 4-byte slots
+    const uint32_t bar_base = base + (uint32_t)p.ring_bytes;        // 8-byte barriers: full[S], empty[S]
+    const uint32_t full_bar = bar_base, empty_bar = bar_base + 8u * S;
+    const uint32_t abort_slot = bar_base + 16u * S;
     uint8_t* gen0 = smem_raw + (base - smem_u32(smem_raw));
-    volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(gen0 + (tmem_slot - base));
     volatile uint32_t* abort_g = reinterpret_cast<volatile uint32_t*>(gen0 + (abort_slot - base));
+    // the accumulator tile overlays the operand ring once every MMA has retired
+    const AccTile acc_tile = {reinterpret_cast<float*>(gen0), p.acc_cols + 4};
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);       // warp-uniform for the compiler (see elect_one_sync)
@@ -107,20 +105,16 @@ k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
     if (tid == 0) {
         for (int s = 0; s < S; ++s) {
             mbar_init(full_bar + 8 * s, p.a_tma ? 2 : 128 + 1);   // 128 producer arrivals (or 1 expect_tx of the A copy) + 1 expect_tx of the weights
-            mbar_init(empty_bar + 8 * s, 1);                       // tcgen05.commit: the stage may be refilled
+            mbar_init(empty_bar + 8 * s, 2);                       // both MMA warpgroups have read the stage
         }
-        mbar_init(tfull_bar, 1);
         *abort_g = 0;
         fence_mbar_init();
     }
-    if (warp == 4) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot_g, 0);
     if (dbg && tid == 0) dbg[1] = clock64();
 
     // ================================================================ main loop roles
+    const __nv_bfloat16* wt = p.wp + (size_t)tile_n * p.num_kb * p.n_mma * 64;     // this n-tile's weight blocks
     if (warp < 4 && p.a_tma) {
         // ---------------- A by the copy engine (linear layers): the 128 x 64 tile of the row-major activation matrix is one
         // cp.async.bulk.tensor.2d into the SWIZZLE_128B stage; rows >= M and columns >= K read as zeros
@@ -133,6 +127,8 @@ k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
                 if (elect_one_sync()) {
                     mbar_arrive_expect_tx(full_bar + 8 * s, UM_A_STAGE);
                     tma_tile_2d(a_base + (uint32_t)s * UM_A_STAGE, &amap, full_bar + 8 * s, kb * UM_BLOCK_K, m0);
+                    mbar_arrive_expect_tx(full_bar + 8 * s, b_stage);
+                    bulk_g2s(b_base + (uint32_t)s * b_stage, wt + (size_t)kb * p.n_mma * 64, b_stage, full_bar + 8 * s);
                 }
                 __syncwarp();
                 if (++s == S) { s = 0; ph ^= 1u; }
@@ -190,6 +186,13 @@ k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
                 cp_async_16(dst, src, ok ? 16u : 0u);
             }
             cp_async_mbar_arrive_noinc(full_bar + 8 * s);
+            if (warp == 0) {                          // B: one bulk copy (TMA engine) per k-block
+                if (elect_one_sync()) {
+                    mbar_arrive_expect_tx(full_bar + 8 * s, b_stage);
+                    bulk_g2s(b_base + (uint32_t)s * b_stage, wt + (size_t)kb * p.n_mma * 64, b_stage, full_bar + 8 * s);
+                }
+                __syncwarp();
+            }
             if (kd) kd[1] = clock64();
             if (++s == S) { s = 0; ph ^= 1; }
             if (p.inc_taps) {
@@ -202,12 +205,11 @@ k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
             }
         }
         if (dbg && tid == 0) dbg[6] = clock64();
-    } else if (warp == 4) {
-        // ---------------- MMA issuer: the whole warp walks the k-blocks (warp-uniform control flow), one elected lane issues
-        // -- under `if (lane == 0)` the compiler moves every descriptor through R2UR in an ELECT loop per MMA (nn_tcgen05.cuh)
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.n_mma >> 3) << 17) |
-                               ((uint32_t)(UM_BLOCK_M >> 4) << 24);
-        const uint64_t d0 = umma_desc_sw128(0u);
+    } else {
+        // ---------------- MMA warpgroups: warpgroup g owns rows 64 g .. 64 g + 63 of the tile (A descriptor + 8 KB)
+        const int wg = (warp - 4) >> 2;
+        const uint64_t d0 = gmma_desc_sw128(0u);
+        float acc[UM_ACC_CH][32];
         int s = 0, fail = 0;
         uint32_t ph = 0u;
 #ifdef NN_KDEBUG
@@ -217,65 +219,50 @@ k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
 #endif
         for (int kb = kb0; kb < kb1; ++kb) {
             if (!mbar_wait(full_bar + 8 * s, ph)) { fail = 2; break; }
-            long long* const kd = (kd0 && lane == 0) ? kd0 + kb * 4 : nullptr;
+            long long* const kd = (kd0 && warp == 4 && lane == 0) ? kd0 + kb * 4 : nullptr;
             if (kd) kd[2] = clock64();
             fence_proxy_async();            // cp.async (generic proxy) writes -> tensor-core (async proxy) reads
-            // (no tcgen05.fence here: the operands come from cp.async / bulk copies, not from tcgen05 ops of other threads)
-            const uint32_t a_s = (a_base + (uint32_t)s * UM_A_STAGE) >> 4, b_s = (b_base + (uint32_t)s * b_stage) >> 4;
-            if (elect_one_sync()) {
-                const uint64_t ad = d0 | (uint64_t)(a_s & 0x3FFFu), bd = d0 | (uint64_t)(b_s & 0x3FFFu);
-                umma_bf16(tmem_base, ad, bd, idesc, kb != kb0);
+            const uint32_t a_s = (a_base + (uint32_t)s * UM_A_STAGE + (uint32_t)wg * 8192u) >> 4, b_s = (b_base + (uint32_t)s * b_stage) >> 4;
+            const uint64_t ad = d0 | (uint64_t)(a_s & 0x3FFFu), bd = d0 | (uint64_t)(b_s & 0x3FFFu);
+            wg_fence();
 #pragma unroll
-                for (int k = 1; k < UM_BLOCK_K / 16; ++k) umma_bf16(tmem_base, ad + 2 * k, bd + 2 * k, idesc, 1u);
-                umma_commit(empty_bar + 8 * s);       // frees the smem stage when these MMAs retire
-            }
+            for (int k = 0; k < UM_BLOCK_K / 16; ++k)       // 64 B rows of the next 64-row chunk of B: + 8 KB = 512 units
+                wg_mma<UM_ACC_CH, 0, 0>(acc, ad + 2 * k, bd + 2 * k, 512u, p.n_mma, (kb != kb0 || k != 0) ? 1 : 0);
+            wg_commit();
+            wg_wait_all();
+            wg_fence_acc(acc);
+            __syncwarp();
+            if ((warp & 3) == 0 && elect_one_sync()) mbar_arrive(empty_bar + 8 * s);      // the stage may be refilled
             __syncwarp();
             if (kd) kd[3] = clock64();
             if (++s == S) { s = 0; ph ^= 1u; }
         }
         if (fail) *abort_g = (uint32_t)fail;
-        if (elect_one_sync()) umma_commit(tfull_bar);                        // accumulators complete
-        __syncwarp();
-        if (dbg && lane == 0) dbg[2] = clock64();
-    } else if (warp == 5) {
-        // ---------------- B loader: one bulk copy (TMA engine) per k-block
-        const __nv_bfloat16* wt = p.wp + (size_t)tile_n * p.num_kb * p.n_mma * 64;
-        int s = 0;
-        uint32_t ph = 1u;
-        for (int kb = kb0; kb < kb1; ++kb) {
-            if (!mbar_wait(empty_bar + 8 * s, ph)) { *abort_g = 3; break; }
-            if (*abort_g) break;
-            if (elect_one_sync()) {
-                mbar_arrive_expect_tx(full_bar + 8 * s, b_stage);
-                bulk_g2s(b_base + (uint32_t)s * b_stage, wt + (size_t)kb * p.n_mma * 64, b_stage, full_bar + 8 * s);
-            }
-            __syncwarp();
-            if (++s == S) { s = 0; ph ^= 1u; }
-        }
+        named_bar_sync(1, 256);              // both warpgroups are done with the operand ring: it becomes the accumulator tile
+        if (!*abort_g && kb1 > kb0) wg_acc_store(acc, acc_tile, 64 * wg, 0, p.n_mma);
+        named_bar_sync(1, 256);
+        if (dbg && tid == 128) dbg[2] = clock64();
     }
-
-    // ================================================================ epilogue (all 8 warps)
-    bool acc_ok = mbar_wait(tfull_bar, 0);
-    tc_fence_after();
-    if (dbg && tid == 0) dbg[3] = clock64();
-    if (!acc_ok || *abort_g) {
-        if (tid == 0) nn_pipeline_abort(p.err_flag, 100 + (int)*abort_g);
+    // ================================================================ epilogue (the 8 MMA warps)
+    if (warp < 4) {
+    } else if (*abort_g) {
+        if (tid == 128) nn_pipeline_abort(p.err_flag, 100 + (int)*abort_g);
     } else if (p.partial) {
         // split-K: raw fp32 accumulators, column-major per n-tile (lanes = consecutive rows: coalesced); the noise
         // epilogue runs in k_splitk_epilogue once all shares are summed.  A share without k-blocks contributes zeros.
-        const int q = warp & 3, half = warp >> 2, row = q * 32 + lane, m = m0 + row;
-        const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
+        const int q = warp & 3, half = (warp - 4) >> 2, row = q * 32 + lane, m = m0 + row;
+        const uint32_t t_lane = (uint32_t)(q * 32) << 16;
         float* dst = p.partial + (((size_t)blockIdx.z * gridDim.y + tile_n) * p.n_mma) * p.m_pad + m;
         for (int ci = half; ci * 16 < p.n_mma; ci += 2) {
             float v[16];
-            tmem_ld16(t_lane + (uint32_t)(ci * 16), v);
+            acc_ld16(acc_tile, t_lane + (uint32_t)(ci * 16), v);
             if (m < p.m_pad) {
 #pragma unroll
                 for (int e = 0; e < 16; ++e) dst[(size_t)(ci * 16 + e) * p.m_pad] = kb1 > kb0 ? v[e] : 0.f;
             }
         }
     } else {
-        const int q = warp & 3, half = warp >> 2;
+        const int q = warp & 3, half = (warp - 4) >> 2;
         const int row = q * 32 + lane;
         const int m = m0 + row;
         const bool row_ok = m < p.M && row < p.rows_tile;
@@ -283,7 +270,7 @@ k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
         int b = 0, pix = 0;
         if (row_ok) { b = m / ohw; pix = m - b * ohw; }
         const size_t out_row = (size_t)b * p.Cout * ohw + pix;
-        const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
+        const uint32_t t_lane = (uint32_t)(q * 32) << 16;
         const bool noise = p.noise_mode != NN_NOISE_NONE;
         float coef = 0.f;
         NnRng rs = {0, 0, 0, 0};
@@ -303,8 +290,8 @@ k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
             for (int ci = half; ci < nchunks; ci += 2) {
                 const int cc = ci * 16;
                 float am[16], as[16];
-                tmem_ld16(t_lane + (uint32_t)(p.main_col + cc), am);
-                if (EPI == 1) tmem_ld16(t_lane + (uint32_t)(p.sig_col + cc), as);
+                acc_ld16(acc_tile, t_lane + (uint32_t)(p.main_col + cc), am);
+                if (EPI == 1) acc_ld16(acc_tile, t_lane + (uint32_t)(p.sig_col + cc), as);
                 if (!row_ok) continue;
                 const int nb = n_base + cc;
                 const int nvalid = min(16, min(p.n_t - cc, p.Cout - nb));
@@ -362,8 +349,8 @@ k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
         for (int ci = half; ci < nchunks; ci += 2) {
             const int cc = ci * 16;
             float am[16], as[16];
-            if (p.main_col >= 0) tmem_ld16(t_lane + (uint32_t)(p.main_col + cc), am);
-            if (noise) tmem_ld16(t_lane + (uint32_t)(p.sig_col + cc), as);
+            if (p.main_col >= 0) acc_ld16(acc_tile, t_lane + (uint32_t)(p.main_col + cc), am);
+            if (noise) acc_ld16(acc_tile, t_lane + (uint32_t)(p.sig_col + cc), as);
             if (!row_ok) continue;
 #pragma unroll
             for (int g4 = 0; g4 < 4; ++g4) {
@@ -405,7 +392,7 @@ k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
         if (EPI == 0 && noise && p.stats) {
             if (p.wsum_col >= 0 && half == 0) {      // external DAC: row sum of x (*) |w| from the colsum row
                 float ws[16];
-                tmem_ld16(t_lane + (uint32_t)p.wsum_col, ws);
+                acc_ld16(acc_tile, t_lane + (uint32_t)p.wsum_col, ws);
                 if (row_ok) s_plain += ws[0] * p.s_scale;
             }
             s_plain = nn_warp_sum(s_plain); s_abs = nn_warp_sum(s_abs); s_max = nn_warp_max(s_max);
@@ -416,11 +403,7 @@ k_conv_umma(const UmmaP p, const __grid_constant__ UmmaAMap amap) {
             }
         }
     }
-    if (dbg && tid == 0) dbg[4] = clock64();
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) { tc_fence_after(); tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols); }
-    if (dbg && tid == 128) { dbg[5] = clock64(); unsigned smid; asm volatile("mov.u32 %0, %%smid;" : "=r"(smid)); dbg[7] = smid; }
+    if (dbg && tid == 128) { dbg[4] = clock64(); unsigned smid; asm volatile("mov.u32 %0, %%smid;" : "=r"(smid)); dbg[7] = smid; }
 }
 
 
@@ -508,14 +491,15 @@ k_splitk_epilogue(const SplitEpiP p) {
 // grid ("virtual" outputs: positions with ow >= OW or oh >= OH are computed and dropped, 12.5 % for 32 -> 28),
 // staged by ONE cp.async.bulk of (128 + (KH-1) W + KW-1) pixels = 4 KB instead of 64 KB of gathered im2col.
 // The whole weight image (taps x rows, 60 KB) stays resident in shared memory, so the CTA is persistent:
-//   warp 0   : bulk-copy issuer (weights once, then the A ring)
-//   warp 1   : tcgen05.mma issuer, one K = 16 MMA per PAIR of taps (LBO = pixel distance of the two taps),
-//              accumulators double-buffered in TMEM (2 x 256 columns)
-//   warps 2+ : epilogue (tcgen05.ld -> scale, Philox/Box-Muller noise -> NCHW stores), overlapping the next
-//              tile's MMAs.  The kernel is bound by the epilogue's instruction issue, not by data movement.
+//   warps 0 .. SH_EPI_WARPS - 1 : epilogue (scale, Philox/Box-Muller noise -> NCHW stores) from a shared-memory
+//              accumulator tile; the first 8 of them are also the two MMA warpgroups (64 tile rows each), one K = 16
+//              wgmma per PAIR of taps (LBO = pixel distance of the two taps), the N columns in 64-wide passes over the
+//              resident operands
+//   last warp : bulk-copy issuer (weights once, then the A ring, which runs ahead of the tiles)
+// The kernel is bound by the epilogue's instruction issue, not by data movement.
 constexpr int SH_MAX_PAIRS = 64;
-constexpr int SH_STAGES = 4;
-constexpr int SH_ACC_STRIDE = 256;                  // TMEM columns between the two accumulator buffers
+constexpr int SH_STAGES = 2;
+constexpr int SH_MAX_N = 256;                       // accumulator columns
 constexpr int SH_POOL_IT = 5;                       // pooled launches: 4-channel groups per epilogue warp (<= 80 channels at 16 warps)
 
 struct ShiftP {
@@ -568,23 +552,25 @@ __device__ __forceinline__ bool shift_tile_live(const ShiftP& p, int t) {
 }
 
 // MODE: 0 plain, 1 noisy (Philox z), 2 noisy with injected z (parity hook); SH_EPI_WARPS: epilogue warps, a
-// multiple of 4 (one TMEM lane quarter per warp % 4)
+// multiple of 4 and at least 8 (one quarter of the tile rows per warp % 4)
 template <int MODE, int SH_EPI_WARPS, bool POOL>
-__global__ void __launch_bounds__((2 + SH_EPI_WARPS) * 32, 1)
+__global__ void __launch_bounds__((1 + SH_EPI_WARPS) * 32, 1)
 k_conv_shift(const ShiftP p) {
     constexpr bool NOISY = MODE != 0;
-    constexpr int SH_THREADS = (2 + SH_EPI_WARPS) * 32;
+    constexpr int SH_THREADS = (1 + SH_EPI_WARPS) * 32;
+    static_assert(SH_EPI_WARPS >= 8 && SH_EPI_WARPS % 4 == 0, "the first 8 epilogue warps are the MMA warpgroups");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 127u) & ~127u;
     const uint32_t b_base = base;
     const uint32_t a_base = b_base + (uint32_t)p.b_bytes;
     const uint32_t bar_base = a_base + (uint32_t)SH_STAGES * (uint32_t)p.a_stage;
     const uint32_t a_full = bar_base, a_empty = bar_base + 8u * SH_STAGES;
-    const uint32_t acc_full = bar_base + 16u * SH_STAGES, acc_empty = acc_full + 16u, b_full = acc_empty + 16u;
-    const uint32_t tmem_slot = b_full + 8u, abort_slot = tmem_slot + 4u, tab_slot = abort_slot + 4u;
+    const uint32_t b_full = bar_base + 16u * SH_STAGES;
+    const uint32_t abort_slot = b_full + 8u, tab_slot = abort_slot + 4u;
     const uint32_t pool_slot = (tab_slot + 4u * SH_MAX_PAIRS + 15u) & ~15u;      // pooling exchange: [warp pair][2][8][16] floats
+    const uint32_t acc_slot = pool_slot + 12u * 1024u;                            // accumulator tile: 128 rows x (n_mma + 4) floats
     uint8_t* gen0 = smem_raw + (base - smem_u32(smem_raw));
-    volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(gen0 + (tmem_slot - base));
+    const AccTile acc_tile = {reinterpret_cast<float*>(gen0 + (acc_slot - base)), p.n_mma + 4};
     volatile uint32_t* abort_g = reinterpret_cast<volatile uint32_t*>(gen0 + (abort_slot - base));
     uint32_t* tap_tab = reinterpret_cast<uint32_t*>(gen0 + (tab_slot - base));   // per tap pair: shift | lbo << 16
 
@@ -597,8 +583,7 @@ k_conv_shift(const ShiftP p) {
         tap_tab[tid] = (uint32_t)sh0 | ((uint32_t)(sh1 - sh0) << 16);
     }
     if (tid == 0) {
-        for (int s = 0; s < SH_STAGES; ++s) { mbar_init(a_full + 8 * s, 1); mbar_init(a_empty + 8 * s, 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(acc_full + 8 * b, 1); mbar_init(acc_empty + 8 * b, SH_EPI_WARPS); }
+        for (int s = 0; s < SH_STAGES; ++s) { mbar_init(a_full + 8 * s, 1); mbar_init(a_empty + 8 * s, 2); }
         mbar_init(b_full, 1);
         *abort_g = 0;
         fence_mbar_init();
@@ -610,16 +595,12 @@ k_conv_shift(const ShiftP p) {
         for (int i = tid; i < n16; i += SH_THREADS) az[i] = make_uint4(0, 0, 0, 0);
         fence_proxy_async();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot_g, 0);
     const int hw = p.H * p.W;
 
-    // loader and MMA issuer: the whole warp walks the tiles (warp-uniform control flow), one elected lane issues the
-    // single-thread instructions (nn_tcgen05.cuh: elect_one_sync)
-    if (warp == 0) {
+    // loader: the whole warp walks the tiles (warp-uniform control flow), one elected lane issues the single-thread
+    // instructions (nn_wgmma.cuh: elect_one_sync)
+    if (warp == SH_EPI_WARPS) {
         if (elect_one_sync()) {
             mbar_arrive_expect_tx(b_full, (uint32_t)p.b_bytes);
             bulk_g2s(b_base, p.wp, (uint32_t)p.b_bytes, b_full);
@@ -643,41 +624,16 @@ k_conv_shift(const ShiftP p) {
             __syncwarp();
             if (++s == SH_STAGES) { s = 0; ph ^= 1u; }
         }
-    } else if (warp == 1) {
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.n_mma >> 3) << 17) |
-                               ((uint32_t)(UM_BLOCK_M >> 4) << 24);
-        bool ok = mbar_wait(b_full, 0);
-        if (!ok) *abort_g = 2;
-        int i = 0, s = 0;
-        uint32_t ph = 0u;
-        const uint64_t bd0 = umma_desc_none(b_base, (uint32_t)p.n_mma, 8u);
-        const uint64_t ad_t = umma_desc_none(0u, 0u, (uint32_t)p.sbo_units);   // A template: start address and LBO vary per tap pair
-        for (int t = blockIdx.x; t < p.n_tiles && ok; t += gridDim.x) {
-            if (!shift_tile_live(p, t)) continue;
-            const int buf = i & 1;
-            if (!mbar_wait(acc_empty + 8 * buf, ((i >> 1) & 1) ^ 1)) { *abort_g = 3; break; }
-            if (!mbar_wait(a_full + 8 * s, ph)) { *abort_g = 4; break; }
-            if (*abort_g) break;
-            tc_fence_after();               // the epilogue warps' tcgen05.ld of this buffer are ordered before the new MMAs
-            if (p.dbg && i < 32 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 0] = clock64();
-            const uint32_t a_s = a_base + (uint32_t)s * p.a_stage;
-            const uint32_t d = tmem_base + (uint32_t)(buf * SH_ACC_STRIDE);
-            if (elect_one_sync()) {
-                for (int j = 0; j < p.n_pairs; ++j) {
-                    const uint32_t e = tap_tab[j];
-                    const uint64_t ad = ad_t | (uint64_t)(((a_s >> 4) + (e & 0xFFFFu)) & 0x3FFFu) | ((uint64_t)((e >> 16) & 0x3FFFu) << 16);
-                    umma_bf16(d, ad, bd0 + (uint64_t)(2 * j * p.n_mma), idesc, j != 0);
-                }
-                umma_commit(a_empty + 8 * s);
-                umma_commit(acc_full + 8 * buf);
-            }
-            __syncwarp();
-            if (p.dbg && i < 32 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 1] = clock64();
-            ++i;
-            if (++s == SH_STAGES) { s = 0; ph ^= 1u; }
-        }
     } else {
-        const int q = warp & 3, jq = (warp - 2) >> 2;
+        // ---- MMA warpgroups (warps 0-7): the tile's accumulators, 64 columns at a time over the resident operands
+        const bool mma_wg = warp < 8;
+        const int wg = warp >> 2;
+        if (mma_wg && !mbar_wait(b_full, 0)) *abort_g = 2;
+        int s = 0;
+        uint32_t ph = 0u;
+        const uint64_t bd0 = gmma_desc_none(b_base, (uint32_t)p.n_mma, 8u);
+        const uint64_t ad_t = gmma_desc_none(0u, 0u, (uint32_t)p.sbo_units);   // A template: start address and LBO vary per tap pair
+        const int q = warp & 3, jq = warp >> 2;
         constexpr int per_q = SH_EPI_WARPS / 4;
         const int ohw = p.OH * p.OW;
         const int ngrp = (p.Cout + 3) >> 2;
@@ -692,14 +648,40 @@ k_conv_shift(const ShiftP p) {
         int i = 0;
         for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
             if (!shift_tile_live(p, t)) continue;
-            const int buf = i & 1;
-            if (!mbar_wait(acc_full + 8 * buf, (i >> 1) & 1)) { *abort_g = 5; break; }
+            if (mma_wg && !*abort_g) {
+                if (!mbar_wait(a_full + 8 * s, ph)) {
+                    *abort_g = 4;
+                } else {
+                    if (p.dbg && i < 32 && warp == 0 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 0] = clock64();
+                    const uint32_t a_s = a_base + (uint32_t)s * p.a_stage + (uint32_t)wg * 128u * (uint32_t)p.sbo_units;   // + 8 row groups
+                    for (int c = 0; 64 * c < p.n_mma; ++c) {
+                        const int n = min(64, p.n_mma - 64 * c);
+                        float acc[1][32];
+                        wg_fence();
+#pragma unroll 1
+                        for (int j = 0; j < p.n_pairs; ++j) {
+                            const uint32_t e = tap_tab[j];
+                            const uint64_t ad = ad_t | (uint64_t)(((a_s >> 4) + (e & 0xFFFFu)) & 0x3FFFu) | ((uint64_t)((e >> 16) & 0x3FFFu) << 16);
+                            wgmma_n<0, 0>(acc[0], ad, bd0 + (uint64_t)(2 * j * p.n_mma + 64 * c), n, j != 0);
+                        }
+                        wg_commit();
+                        wg_wait_all();
+                        wg_fence_regs<32>(acc[0]);
+                        wg_acc_store(acc, acc_tile, 64 * wg, 64 * c, n);
+                    }
+                    __syncwarp();
+                    if ((warp & 3) == 0 && elect_one_sync()) mbar_arrive(a_empty + 8 * s);     // the A stage may be refilled
+                    __syncwarp();
+                    if (p.dbg && i < 32 && warp == 0 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 1] = clock64();
+                }
+                if (++s == SH_STAGES) { s = 0; ph ^= 1u; }
+            }
+            named_bar_sync(1, SH_EPI_WARPS * 32);          // the tile's accumulators are in the shared-memory tile
             if (*abort_g) break;
-            tc_fence_after();
-            if (p.dbg && i < 32 && warp == 2 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 2] = clock64();
+            if (p.dbg && i < 32 && warp == 0 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 2] = clock64();
             int b, ih, iw;
             bool row_ok;
-            if (p.blk) {        // block tile: TMEM lane = 8 * (row in tile) + column, so a warp holds 4 rows x 8 columns
+            if (p.blk) {        // block tile: tile row = 8 * (image row in tile) + column, so a warp holds 4 rows x 8 columns
                 int r0, c0;
                 shift_tile_v0(p, t, b, r0, c0);
                 ih = r0 + q * 4 + (lane >> 3); iw = c0 + (lane & 7);
@@ -716,7 +698,7 @@ k_conv_shift(const ShiftP p) {
             const size_t out_row = (size_t)b * p.Cout * ohw + pix;
             float* const out_main = (NOISY ? p.y_noisy : p.y) + out_row;
             float* const out_y = (NOISY && p.y) ? p.y + out_row : nullptr;
-            const uint32_t t_lane = tmem_base + (uint32_t)(buf * SH_ACC_STRIDE) + ((uint32_t)(q * 32) << 16);
+            const uint32_t t_lane = (uint32_t)(q * 32) << 16;
             if (POOL) {
                 // Fused MaxPool2d(2,2) on block tiles: the window of lane l is {l, l^1, l^8, l^9} (columns iw, iw+1 of rows
                 // ih, ih+1).  The four lanes of a window SHARE the work: the lane at window position w finalizes channel w of
@@ -767,12 +749,12 @@ k_conv_shift(const ShiftP p) {
 #pragma unroll
                 for (int it = 0; it < SH_POOL_IT; ++it) {
                     if (MODE == 1 && (it & 1) == 0 && it + 1 < SH_POOL_IT - 1) {
-                        // two fixed groups per trip where there are two: one TMEM wait, two independent Philox chains
+                        // two fixed groups per trip where there are two: one accumulator read, two independent Philox chains
                         if (it + 1 < n_fix) {
                             if (!warp_live) continue;
                             const int ga = jq + it * per_q, gb = ga + per_q;
                             float am[4], as[4], bm[4], bs[4], za[4], zb[4], va[4], vb[4];
-                            tmem_ld4x4(t_lane + (uint32_t)(p.main_col + ga * 4), t_lane + (uint32_t)(p.sig_col + ga * 4),
+                            acc_ld4x4(acc_tile, t_lane + (uint32_t)(p.main_col + ga * 4), t_lane + (uint32_t)(p.sig_col + ga * 4),
                                        t_lane + (uint32_t)(p.main_col + gb * 4), t_lane + (uint32_t)(p.sig_col + gb * 4), am, as, bm, bs);
                             nn_normal4(rs, grp_row + (uint64_t)ga, za);
                             nn_normal4(rs, grp_row + (uint64_t)gb, zb);
@@ -790,8 +772,8 @@ k_conv_shift(const ShiftP p) {
                     else { g4 = g_extra; if (g4 >= ngrp || (i % per_q) != jq) continue; }
                     if (!warp_live) continue;
                     float am[4], as[4];
-                    if (NOISY) tmem_ld4x2(t_lane + (uint32_t)(p.main_col + g4 * 4), t_lane + (uint32_t)(p.sig_col + g4 * 4), am, as);
-                    else tmem_ld4(t_lane + (uint32_t)(p.main_col + g4 * 4), am);
+                    if (NOISY) acc_ld4x2(acc_tile, t_lane + (uint32_t)(p.main_col + g4 * 4), t_lane + (uint32_t)(p.sig_col + g4 * 4), am, as);
+                    else acc_ld4(acc_tile, t_lane + (uint32_t)(p.main_col + g4 * 4), am);
                     const int nb = g4 * 4;
                     float z[4] = {0.f, 0.f, 0.f, 0.f};
                     if (MODE == 1) nn_normal4(rs, grp_row + (uint64_t)g4, z);
@@ -805,8 +787,8 @@ k_conv_shift(const ShiftP p) {
             {
             auto one_group = [&](int g4) {
                 float am[4], as[4];
-                if (NOISY) tmem_ld4x2(t_lane + (uint32_t)(p.main_col + g4 * 4), t_lane + (uint32_t)(p.sig_col + g4 * 4), am, as);
-                else tmem_ld4(t_lane + (uint32_t)(p.main_col + g4 * 4), am);
+                if (NOISY) acc_ld4x2(acc_tile, t_lane + (uint32_t)(p.main_col + g4 * 4), t_lane + (uint32_t)(p.sig_col + g4 * 4), am, as);
+                else acc_ld4(acc_tile, t_lane + (uint32_t)(p.main_col + g4 * 4), am);
                 if (!row_ok) return;
                 const int nb = g4 * 4;
                 float z[4];
@@ -845,10 +827,10 @@ k_conv_shift(const ShiftP p) {
             for (int g4 = (jq + i) % per_q; g4 < ngrp; g4 += 2 * per_q) {
                 const int g4b = g4 + per_q;
                 if (hot && g4b * 4 + 4 <= p.Cout) {
-                    // two groups per trip: one TMEM wait for both, and two independent Philox / Box-Muller chains for the
+                    // two groups per trip: one accumulator read for both, and two independent Philox / Box-Muller chains for the
                     // scheduler to interleave (the epilogue is latency-bound: one chain per warp left it at ~0.3 IPC)
                     float am[4], as[4], bm[4], bs[4];
-                    tmem_ld4x4(t_lane + (uint32_t)(p.main_col + g4 * 4), t_lane + (uint32_t)(p.sig_col + g4 * 4),
+                    acc_ld4x4(acc_tile, t_lane + (uint32_t)(p.main_col + g4 * 4), t_lane + (uint32_t)(p.sig_col + g4 * 4),
                                t_lane + (uint32_t)(p.main_col + g4b * 4), t_lane + (uint32_t)(p.sig_col + g4b * 4), am, as, bm, bs);
                     if (!row_ok) continue;
                     float za[4], zb[4];
@@ -869,10 +851,8 @@ k_conv_shift(const ShiftP p) {
                 if (g4b < ngrp) one_group(g4b);
             }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(acc_empty + 8 * buf);
-            if (p.dbg && i < 32 && warp == 2 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 3] = clock64();
+            named_bar_sync(1, SH_EPI_WARPS * 32);          // the accumulator tile may be overwritten
+            if (p.dbg && i < 32 && warp == 0 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 3] = clock64();
             ++i;
         }
         if (POOL && p.stat_partial) {
@@ -887,10 +867,10 @@ k_conv_shift(const ShiftP p) {
                     if (o == 8) continue;
                     a1 += __shfl_xor_sync(0xffffffffu, a1, o); a2 += __shfl_xor_sync(0xffffffffu, a2, o);
                 }
-                if ((lane & ~9) == 0) { ssum[(((warp - 2) * SH_POOL_IT + it) * 4 + w) * 2] = a1; ssum[(((warp - 2) * SH_POOL_IT + it) * 4 + w) * 2 + 1] = a2; }
+                if ((lane & ~9) == 0) { ssum[((warp * SH_POOL_IT + it) * 4 + w) * 2] = a1; ssum[((warp * SH_POOL_IT + it) * 4 + w) * 2 + 1] = a2; }
             }
             asm volatile("bar.sync 1, %0;" ::"r"(SH_EPI_WARPS * 32) : "memory");
-            const int et = tid - 64;                                               // epilogue thread index
+            const int et = tid;                                                    // epilogue thread index
             if (et < p.Cout) {
                 const int g4 = et >> 2, j = et & 3, n_fix = ngrp / per_q;
                 double d1 = 0.0, d2 = 0.0;
@@ -920,14 +900,12 @@ k_conv_shift(const ShiftP p) {
                 if (et < p.Cout) bn_finalize_channel(p.stat_partial + (size_t)et * 2, (int)gridDim.x, (int64_t)p.Cout * 2, et, p.fin);
                 if (et == 0) { *p.stat_ticket = 0u; if (p.zero_out) *p.zero_out = 0.f; }
             }
-        } else if (p.zero_out && blockIdx.x == 0 && tid == 64) {
+        } else if (p.zero_out && blockIdx.x == 0 && tid == 0) {
             *p.zero_out = 0.f;
         }
     }
-    tc_fence_before();
     __syncthreads();
     if (*abort_g && tid == 0) nn_pipeline_abort(p.err_flag, 200 + (int)*abort_g);
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
 }
 
 // ------------------------------------------------------------------ operand packing
@@ -1144,8 +1122,8 @@ k_pack_w_batch(const PackJobs jobs) {
     pack_w_job(jobs.j[blockIdx.y], blockIdx.x * (int64_t)blockDim.x + threadIdx.x, (int64_t)gridDim.x * blockDim.x);
 }
 
-// ------------------------------------------------------------------ wgrad on tcgen05 (MN-major operands)
-//   D[n, kcol] = sum_m gy[m, n] * im2col(x)[m, kcol]      n = output channel (128 TMEM lanes),
+// ------------------------------------------------------------------ wgrad on the tensor cores (MN-major operands)
+//   D[n, kcol] = sum_m gy[m, n] * im2col(x)[m, kcol]      n = output channel (128 tile rows),
 //   kcol = tap * Cp + c (up to 256 accumulator columns per CTA), reduction over output pixels m.
 // Both operands are read from NHWC bf16 packs, i.e. contiguous along their M / N dimension: they are staged
 // as MN-major SWIZZLE_128B tiles  [MN atom of 64 elements][64 reduction rows][128 B]  (LBO = MN-atom stride,
@@ -1156,13 +1134,13 @@ struct WgUP {
     int KH, KW, stride, pad, OH, OW;
     int Mpix, Cout, Coutp;           // gyp [Mpix, Coutp]    (grad_output, NHWC bf16)
     int Ktot, NT, ktot_pad;          // Ktot = KH*KW*Cp, NT = accumulator columns per CTA, ktot_pad = tiles * NT
-    int num_kb, kb_per_split, stages, tmem_cols;
+    int num_kb, kb_per_split, stages;
     const __nv_bfloat16 *xp, *gyp;
     float* partial;                  // [splits][Cout][ktot_pad]
     int* err_flag;
 };
 
-__global__ void __launch_bounds__(UM_THREADS, 2)
+__global__ void __launch_bounds__(UM_THREADS, 1)
 k_wgrad_umma(const WgUP p) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -1170,10 +1148,9 @@ k_wgrad_umma(const WgUP p) {
     const uint32_t b_stage = (uint32_t)p.NT * 128u;                 // 64 rows x NT bf16
     const uint32_t a_base = base, b_base = base + (uint32_t)S * UM_A_STAGE;
     const uint32_t bar_base = b_base + (uint32_t)S * b_stage;
-    const uint32_t full_bar = bar_base, empty_bar = bar_base + 8u * S, tfull_bar = bar_base + 16u * S;
-    const uint32_t tmem_slot = tfull_bar + 8, abort_slot = tmem_slot + 4, tab_base = (abort_slot + 4 + 15u) & ~15u;
+    const uint32_t full_bar = bar_base, empty_bar = bar_base + 8u * S;
+    const uint32_t abort_slot = bar_base + 16u * S, tab_base = (abort_slot + 4 + 15u) & ~15u;
     uint8_t* gen0 = smem_raw + (base - smem_u32(smem_raw));
-    volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(gen0 + (tmem_slot - base));
     volatile uint32_t* abort_g = reinterpret_cast<volatile uint32_t*>(gen0 + (abort_slot - base));
     int4* tab = reinterpret_cast<int4*>(gen0 + (tab_base - base));  // per 16-byte column chunk: {kh, kw, c0, valid}
 
@@ -1186,8 +1163,7 @@ k_wgrad_umma(const WgUP p) {
     const int nchunk = p.NT >> 3;
 
     if (tid == 0) {
-        for (int s = 0; s < S; ++s) { mbar_init(full_bar + 8 * s, 128); mbar_init(empty_bar + 8 * s, 1); }
-        mbar_init(tfull_bar, 1);
+        for (int s = 0; s < S; ++s) { mbar_init(full_bar + 8 * s, 128); mbar_init(empty_bar + 8 * s, 2); }
         *abort_g = 0;
         fence_mbar_init();
     }
@@ -1197,11 +1173,7 @@ k_wgrad_umma(const WgUP p) {
         const int kh = tap / p.KW, kw = tap - kh * p.KW;
         tab[q] = make_int4(kh, kw, c0, (kcol < p.Ktot) ? 1 : 0);
     }
-    if (warp == 4) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot_g, 0);
 
     if (warp < 4) {
         // Lane mapping (as in the forward producer): consecutive lanes fetch consecutive 16-byte chunks of one
@@ -1258,60 +1230,53 @@ k_wgrad_umma(const WgUP p) {
             }
             cp_async_mbar_arrive_noinc(full_bar + 8 * s);
         }
-    } else if (warp == 4) {
-        // MN-major A and B (bits 15, 16), bf16 x bf16 -> f32, M = 128, N = NT; whole warp walks, elected lane issues
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) |
-                               ((uint32_t)(p.NT >> 3) << 17) | ((uint32_t)(UM_BLOCK_M >> 4) << 24);
-        const uint64_t d0 = umma_desc_sw128(0u) | ((uint64_t)((64u * 128u) >> 4) << 16);        // LBO = MN-atom stride = 8192 B
-        int s = 0;
+    } else {
+        // MMA warpgroups: MN-major A and B, bf16 x bf16 -> fp32; warpgroup g owns rows (output channels) 64 g .. 64 g + 63 =
+        // the second 64-element MN atom of A (+ 8 KB); the 64-column chunks of N are B's MN atoms (LBO = 8192 B)
+        const int wg = (warp - 4) >> 2;
+        const uint64_t d0 = gmma_desc(0u, (64u * 128u) >> 4, 1024u >> 4, 1u);
+        float acc[UM_ACC_CH][32];
+        int s = 0, fail = 0;
         uint32_t ph = 0u;
         for (int i = 0; i < nkb; ++i) {
-            if (!mbar_wait(full_bar + 8 * s, ph)) { *abort_g = 2; break; }
+            if (!mbar_wait(full_bar + 8 * s, ph)) { fail = 2; break; }
             fence_proxy_async();
-            // (no tcgen05.fence per k-block, see k_conv_umma)
-            const uint32_t a_s = (a_base + (uint32_t)s * UM_A_STAGE) >> 4, b_s = (b_base + (uint32_t)s * b_stage) >> 4;
-            if (elect_one_sync()) {
-                const uint64_t ad = d0 | (uint64_t)(a_s & 0x3FFFu), bd = d0 | (uint64_t)(b_s & 0x3FFFu);
-                umma_bf16(tmem_base, ad, bd, idesc, i != 0);
+            const uint32_t a_s = (a_base + (uint32_t)s * UM_A_STAGE + (uint32_t)wg * 8192u) >> 4, b_s = (b_base + (uint32_t)s * b_stage) >> 4;
+            const uint64_t ad = d0 | (uint64_t)(a_s & 0x3FFFu), bd = d0 | (uint64_t)(b_s & 0x3FFFu);
+            wg_fence();
 #pragma unroll
-                for (int k = 1; k < 4; ++k)                                  // 16 reduction rows = 2048 B = 128 units
-                    umma_bf16(tmem_base, ad + 128 * k, bd + 128 * k, idesc, 1u);
-                umma_commit(empty_bar + 8 * s);
-            }
+            for (int k = 0; k < 4; ++k)                                  // 16 reduction rows = 2048 B = 128 units
+                wg_mma<UM_ACC_CH, 1, 1>(acc, ad + 128 * k, bd + 128 * k, 512u, p.NT, (i | k) != 0 ? 1 : 0);
+            wg_commit();
+            wg_wait_all();
+            wg_fence_acc(acc);
+            __syncwarp();
+            if ((warp & 3) == 0 && elect_one_sync()) mbar_arrive(empty_bar + 8 * s);
             __syncwarp();
             if (++s == S) { s = 0; ph ^= 1u; }
         }
-        if (elect_one_sync()) umma_commit(tfull_bar);
-        __syncwarp();
-    }
-
-    bool acc_ok = mbar_wait(tfull_bar, 0);
-    tc_fence_after();
-    if (!acc_ok || *abort_g) {
-        if (tid == 0) nn_pipeline_abort(p.err_flag, 200 + (int)*abort_g);
-    } else {
-        const int q = warp & 3, half = warp >> 2;
-        const int n = tile_n * 128 + q * 32 + lane;
-        const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-        float* out = p.partial + ((size_t)split * p.Cout + (n < p.Cout ? n : 0)) * p.ktot_pad + (size_t)tile_k * p.NT;
-        const int nchunks16 = p.NT >> 4;
-        for (int ci = half; ci < nchunks16; ci += 2) {
-            float v[16];
-            if (nkb > 0) tmem_ld16(t_lane + (uint32_t)(ci * 16), v);
-            else {
+        if (fail) *abort_g = (uint32_t)fail;
+        if (*abort_g) {
+            if (warp == 4 && lane == 0) nn_pipeline_abort(p.err_flag, 200 + (int)*abort_g);
+        } else {
+            // rows = output channels, columns = this CTA's (tap, channel) columns: partial[split][n][tile_k * NT + col]
+            const int wt = tid & 127;
+            const int n0 = tile_n * 128 + 64 * wg + 16 * (wt >> 5) + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
-                for (int e = 0; e < 16; ++e) v[e] = 0.f;
-            }
-            if (n < p.Cout) {
-                float4* o4 = reinterpret_cast<float4*>(out + ci * 16);
+            for (int h = 0; h < 2; ++h) {
+                const int n = n0 + 8 * h;
+                if (n >= p.Cout) continue;
+                float* out = p.partial + ((size_t)split * p.Cout + n) * p.ktot_pad + (size_t)tile_k * p.NT + c0;
 #pragma unroll
-                for (int e = 0; e < 4; ++e) o4[e] = make_float4(v[4 * e], v[4 * e + 1], v[4 * e + 2], v[4 * e + 3]);
+                for (int c = 0; c < UM_ACC_CH; ++c)
+#pragma unroll
+                    for (int j = 0; j < 8; ++j)
+                        if (64 * c + 8 * j < p.NT)
+                            *reinterpret_cast<float2*>(out + 64 * c + 8 * j) =
+                                nkb > 0 ? make_float2(acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]) : make_float2(0.f, 0.f);
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) { tc_fence_after(); tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols); }
 }
 
 // ================================================================== shift-GEMM wgrad (narrow-input layers)
@@ -1324,17 +1289,17 @@ k_wgrad_umma(const WgUP p) {
 //   * grad_output comes in the PLANES layout [channel chunk][virtual pixel][8] on the INPUT pixel grid (zeros at
 //     positions that are not outputs; written once per step by the stage backward, NN_PACK_SHIFT), so a chunk
 //     of 128 pixels is one contiguous 2 KB slab per channel chunk and the M atoms are the planes.
-// Nothing is gathered: per 128-pixel reduction chunk the loader issues 9 + 1 bulk copies (23 KB), the MMA
-// thread 8 x KH MMAs, and the CTA (persistent, split over the reduction) keeps its accumulators in TMEM until the
-// end: HBM-bound (gy 75 MB at batch 512) instead of gather-bound.
+// Nothing is gathered: per 128-pixel reduction chunk the loader issues 9 + 1 bulk copies (23 KB), the two MMA
+// warpgroups (64 output channels each) 8 x KH wgmmas, and the CTA (persistent, split over the reduction) keeps its
+// accumulators in registers until the end -- kernel rows in passes of up to 256 columns (one pass for 5 x 5).
 constexpr int WS_KP = 128;                 // reduction pixels per stage
 constexpr int WS_MAX_STAGES = 6;
-constexpr int WS_THREADS = 192;            // warp 0 loader, warp 1 MMA, warps 2-5 epilogue
+constexpr int WS_THREADS = 288;            // warps 0-7 MMA warpgroups (then the epilogue), warp 8 loader
 
 struct WgShiftP {
     int H, W, OH, OW, KH, KW, Cout;
     int n_planes, n_row, n_chunks;          // gy channel chunks, accumulator columns per kernel row, reduction chunks
-    int b_pixels, a_stage, b_stage, stages, tmem_cols, order;
+    int b_pixels, a_stage, b_stage, stages;
     long long total_pixels, plane_stride;   // plane_stride = total_pixels rounded up to WS_KP (zeros in the padding)
     const __nv_bfloat16 *xp, *gyv;
     float* partial;                         // [gridDim.x][Cout][row_pitch], column tap * 8 + c
@@ -1342,12 +1307,6 @@ struct WgShiftP {
     int* err_flag;
     long long* dbg;                         // optional [cta][32 chunks][4]: before wait, operands landed, MMAs issued
 };
-
-// SWIZZLE_NONE MN-major descriptor: sbo = distance between 8-element MN atoms, lbo = distance between 8-row
-// reduction groups (16-byte units)
-__device__ __forceinline__ uint64_t umma_desc_none_mn(uint32_t smem_addr, uint32_t lbo_units, uint32_t sbo_units) {
-    return umma_desc_none(smem_addr, lbo_units, sbo_units);
-}
 
 __device__ __forceinline__ bool wgshift_chunk_live(const WgShiftP& p, int t) {
     const long long v0 = (long long)t * WS_KP;
@@ -1359,27 +1318,26 @@ __device__ __forceinline__ bool wgshift_chunk_live(const WgShiftP& p, int t) {
     return (int)((v0 - b0 * hw) / p.W) < p.OH;
 }
 
-__global__ void __launch_bounds__(WS_THREADS, 2)
+// NROW: accumulator columns per kernel row (KW taps x 8 channels, padded to 16)
+template <int NROW>
+__global__ void __launch_bounds__(WS_THREADS, 1)
 k_wgrad_shift(const WgShiftP p) {
+    constexpr int KHB = 256 / NROW;          // kernel rows per pass (registers: KHB * NROW / 2 <= 128 per thread)
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 127u) & ~127u;
     const int WS_STAGES = p.stages;
     const uint32_t b_base = base;
     const uint32_t a_base = b_base + (uint32_t)WS_STAGES * (uint32_t)p.b_stage;
     const uint32_t bar_base = a_base + (uint32_t)WS_STAGES * (uint32_t)p.a_stage + 16u * WS_KP * 16u;   // + phantom planes
-    const uint32_t full_bar = bar_base, empty_bar = bar_base + 8u * WS_MAX_STAGES, acc_bar = bar_base + 16u * WS_MAX_STAGES;
-    const uint32_t tmem_slot = acc_bar + 8u, abort_slot = tmem_slot + 4u, work_slot = abort_slot + 4u;
+    const uint32_t full_bar = bar_base, empty_bar = bar_base + 8u * WS_MAX_STAGES;
+    const uint32_t abort_slot = bar_base + 16u * WS_MAX_STAGES;
     uint8_t* gen0 = smem_raw + (base - smem_u32(smem_raw));
-    volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(gen0 + (tmem_slot - base));
     volatile uint32_t* abort_g = reinterpret_cast<volatile uint32_t*>(gen0 + (abort_slot - base));
-    volatile uint32_t* work_g = reinterpret_cast<volatile uint32_t*>(gen0 + (work_slot - base));
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);       // warp-uniform for the compiler (see elect_one_sync)
     if (tid == 0) {
-        for (int s = 0; s < WS_STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 1); }
-        mbar_init(acc_bar, 1);
+        for (int s = 0; s < WS_STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, 2); }
         *abort_g = 0;
-        *work_g = 0;
         fence_mbar_init();
     }
     {   // zero both rings once: x pixels past the end of the pack are never loaded but are multiplied by zero
@@ -1389,108 +1347,85 @@ k_wgrad_shift(const WgShiftP p) {
         for (int i = tid; i < n16; i += WS_THREADS) z[i] = make_uint4(0, 0, 0, 0);
         fence_proxy_async();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = __shfl_sync(0xffffffffu, *tmem_slot_g, 0);
 
-    if (warp == 0) {
+    if (warp == 8) {
         int s = 0;
         uint32_t ph = 1u;
-        for (int t = blockIdx.x; t < p.n_chunks; t += gridDim.x) {
-            if (!wgshift_chunk_live(p, t)) continue;
-            if (!mbar_wait(empty_bar + 8 * s, ph)) { *abort_g = 1; break; }
-            if (*abort_g) break;
-            const long long v0 = (long long)t * WS_KP;
-            const long long pa = WS_KP;              // planes are padded to a multiple of WS_KP pixels
-            long long pb = p.total_pixels - v0;
-            if (pb > p.b_pixels) pb = p.b_pixels;
-            if (elect_one_sync()) {
-                mbar_arrive_expect_tx(full_bar + 8 * s, (uint32_t)(pa * 16 * p.n_planes + pb * 16));
-                bulk_g2s(b_base + (uint32_t)s * p.b_stage, p.xp + v0 * 8, (uint32_t)pb * 16u, full_bar + 8 * s);
-                for (int c = 0; c < p.n_planes; ++c)
-                    bulk_g2s(a_base + (uint32_t)s * p.a_stage + (uint32_t)c * (WS_KP * 16u),
-                             p.gyv + ((long long)c * p.plane_stride + v0) * 8, (uint32_t)pa * 16u, full_bar + 8 * s);
+        for (int kh0 = 0; kh0 < p.KH; kh0 += KHB)              // one sweep over the reduction per pass
+            for (int t = blockIdx.x; t < p.n_chunks; t += gridDim.x) {
+                if (!wgshift_chunk_live(p, t)) continue;
+                if (!mbar_wait(empty_bar + 8 * s, ph)) { *abort_g = 1; break; }
+                if (*abort_g) break;
+                const long long v0 = (long long)t * WS_KP;
+                const long long pa = WS_KP;              // planes are padded to a multiple of WS_KP pixels
+                long long pb = p.total_pixels - v0;
+                if (pb > p.b_pixels) pb = p.b_pixels;
+                if (elect_one_sync()) {
+                    mbar_arrive_expect_tx(full_bar + 8 * s, (uint32_t)(pa * 16 * p.n_planes + pb * 16));
+                    bulk_g2s(b_base + (uint32_t)s * p.b_stage, p.xp + v0 * 8, (uint32_t)pb * 16u, full_bar + 8 * s);
+                    for (int c = 0; c < p.n_planes; ++c)
+                        bulk_g2s(a_base + (uint32_t)s * p.a_stage + (uint32_t)c * (WS_KP * 16u),
+                                 p.gyv + ((long long)c * p.plane_stride + v0) * 8, (uint32_t)pa * 16u, full_bar + 8 * s);
+                }
+                __syncwarp();
+                if (++s == WS_STAGES) { s = 0; ph ^= 1u; }
             }
-            __syncwarp();
-            if (++s == WS_STAGES) { s = 0; ph ^= 1u; }
-        }
-    } else if (warp == 1) {
-        // MN-major A and B (bits 15, 16), bf16 x bf16 -> fp32, M = 128, N = n_row; whole warp walks, elected lane issues
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) |
-                               ((uint32_t)(p.n_row >> 3) << 17) | ((uint32_t)(UM_BLOCK_M >> 4) << 24);
-        int i = 0, s = 0;
+    } else {
+        // MN-major A (grad_output planes: SBO = plane stride, LBO = 8 pixels) and B (x: the taps of a kernel row are MN atoms
+        // one pixel apart), bf16 x bf16 -> fp32; warpgroup g owns output channels 64 g .. 64 g + 63 (planes 8 g ..)
+        const int wg = warp >> 2, wt = tid & 127;
+        const int n0 = 64 * wg + 16 * (wt >> 5) + (lane >> 2), c0 = 2 * (lane & 3);
+        int s = 0;
         uint32_t ph = 0u;
-        for (int t = blockIdx.x; t < p.n_chunks; t += gridDim.x) {
-            if (!wgshift_chunk_live(p, t)) continue;
-            if (p.dbg && i < 32 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 0] = clock64();
-            if (!mbar_wait(full_bar + 8 * s, ph)) { *abort_g = 2; break; }
-            if (*abort_g) break;
-            // (no tcgen05.fence per chunk, see k_conv_umma)
-            if (p.dbg && i < 32 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 1] = clock64();
-            const uint64_t ad0 = umma_desc_none_mn(a_base + (uint32_t)s * p.a_stage, 8u, (uint32_t)WS_KP);
-            const uint64_t bd0 = umma_desc_none_mn(b_base + (uint32_t)s * p.b_stage, 8u, 1u);
-            if (elect_one_sync()) {
-                if (p.order) {
+        for (int kh0 = 0; kh0 < p.KH && !*abort_g; kh0 += KHB) {
+            const int nkh = min(KHB, p.KH - kh0);
+            float acc[KHB][NROW / 2];
+            int i = 0;
+            for (int t = blockIdx.x; t < p.n_chunks; t += gridDim.x) {
+                if (!wgshift_chunk_live(p, t)) continue;
+                if (!mbar_wait(full_bar + 8 * s, ph)) { *abort_g = 2; break; }
+                if (*abort_g) break;
+                const uint64_t ad0 = gmma_desc_none(a_base + (uint32_t)s * p.a_stage + (uint32_t)wg * 8u * (WS_KP * 16u), 8u, (uint32_t)WS_KP);
+                const uint64_t bd0 = gmma_desc_none(b_base + (uint32_t)s * p.b_stage + (uint32_t)kh0 * (uint32_t)p.W * 16u, 8u, 1u);
+                wg_fence();
 #pragma unroll 1
-                    for (int kh = 0; kh < p.KH; ++kh)
-                        for (int k = 0; k < WS_KP / 16; ++k)
-                            umma_bf16(tmem_base + (uint32_t)(kh * p.n_row), ad0 + (uint64_t)(k * 16),
-                                      bd0 + (uint64_t)(k * 16 + kh * p.W), idesc, (i | k) != 0);
-                } else {
-#pragma unroll 1
-                    for (int k = 0; k < WS_KP / 16; ++k) {
-                        for (int kh = 0; kh < p.KH; ++kh)
-                            umma_bf16(tmem_base + (uint32_t)(kh * p.n_row), ad0 + (uint64_t)(k * 16),
-                                      bd0 + (uint64_t)(k * 16 + kh * p.W), idesc, (i | k) != 0);
-                    }
-                }
-                umma_commit(empty_bar + 8 * s);
-            }
-            __syncwarp();
-            if (p.dbg && i < 32 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 2] = clock64();
-            ++i;
-            if (++s == WS_STAGES) { s = 0; ph ^= 1u; }
-        }
-        if (lane == 0) *work_g = (uint32_t)i;
-        if (elect_one_sync()) umma_commit(acc_bar);
-        __syncwarp();
-    }
-    if (warp >= 2) {
-        // epilogue: accumulator rows = output channels; columns (kh, kw, c) -> partial[cta][n][tap * 8 + c]
-        const bool ok = mbar_wait(acc_bar, 0);
-        tc_fence_after();
-        if (!ok) *abort_g = 3;
-        const int q = warp & 3;
-        const int n = q * 32 + lane;
-        float* dst = p.partial + ((size_t)blockIdx.x * p.Cout + n) * p.row_pitch;      // row pitch 256: k_wgrad_tma_reduce's tail format
-        const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-        if (ok && !*abort_g) {
-            for (int kh = 0; kh < p.KH; ++kh)
-                for (int kw = 0; kw < p.KW; kw += 2) {
-                    float v[16];
-                    tmem_ld16(t_lane + (uint32_t)(kh * p.n_row + kw * 8), v);     // two taps (the second may be the extra one)
-                    if (*work_g == 0) {                                            // a CTA without live chunks contributes zeros
+                for (int k = 0; k < WS_KP / 16; ++k) {
 #pragma unroll
-                        for (int e = 0; e < 16; ++e) v[e] = 0.f;
-                    }
-                    if (n < p.Cout) {
-                        float4* d4 = reinterpret_cast<float4*>(dst + (kh * p.KW + kw) * 8);
-                        d4[0] = make_float4(v[0], v[1], v[2], v[3]);
-                        d4[1] = make_float4(v[4], v[5], v[6], v[7]);
-                        if (kw + 1 < p.KW) {
-                            d4[2] = make_float4(v[8], v[9], v[10], v[11]);
-                            d4[3] = make_float4(v[12], v[13], v[14], v[15]);
-                        }
-                    }
+                    for (int j = 0; j < KHB; ++j)
+                        if (j < nkh)
+                            wgmma_c<NROW, 1, 1>(acc[j], ad0 + (uint64_t)(k * 16), bd0 + (uint64_t)(k * 16 + j * p.W), (i | k) != 0);
                 }
+                wg_commit();
+                wg_wait_all();
+#pragma unroll
+                for (int j = 0; j < KHB; ++j) wg_fence_regs<NROW / 2>(acc[j]);
+                __syncwarp();
+                if ((warp & 3) == 0 && elect_one_sync()) mbar_arrive(empty_bar + 8 * s);
+                __syncwarp();
+                ++i;
+                if (++s == WS_STAGES) { s = 0; ph ^= 1u; }
+            }
+            if (*abort_g) break;
+            // accumulator rows = output channels; columns (kh, kw, c) -> partial[cta][n][tap * 8 + c] (row pitch 256:
+            // k_wgrad_tma_reduce's tail format); a CTA without live chunks contributes zeros
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int n = n0 + 8 * h;
+                if (n >= p.Cout) continue;
+                float* dst = p.partial + ((size_t)blockIdx.x * p.Cout + n) * p.row_pitch + c0;
+#pragma unroll
+                for (int j = 0; j < KHB; ++j)
+#pragma unroll
+                    for (int kw = 0; kw < NROW / 8; ++kw)
+                        if (j < nkh && kw < p.KW)
+                            *reinterpret_cast<float2*>(dst + ((kh0 + j) * p.KW + kw) * 8) =
+                                i > 0 ? make_float2(acc[j][4 * kw + 2 * h], acc[j][4 * kw + 2 * h + 1]) : make_float2(0.f, 0.f);
+            }
         }
     }
-    tc_fence_before();
     __syncthreads();
     if (*abort_g && tid == 0) nn_pipeline_abort(p.err_flag, 300 + (int)*abort_g);
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols); }
 }
 
 // grad_output NCHW fp32 -> planes layout on the input pixel grid (zeros elsewhere), for callers that did not
@@ -1649,7 +1584,7 @@ k_wgrad_tma_reduce(const WgRedP p) {
 
 // ------------------------------------------------------------------ host-side planning
 struct Plan {
-    int Cp, K_total, num_kb, n_tiles, n_t, n_mma, tmem_cols, stages, main_col, sig_col, wsum_col;
+    int Cp, K_total, num_kb, n_tiles, n_t, n_mma, acc_cols, stages, main_col, sig_col, wsum_col, ring_bytes;
     size_t xp_bytes, wp_bytes, smem_bytes;
 };
 
@@ -1665,7 +1600,7 @@ static Plan make_plan(int Cin_k, int KHW, int n_out, bool has_main, bool has_sig
     const int max_nt = has_sigma ? (has_main ? env_max_nt : 248) : 256;
     pl.n_tiles = (n_out + max_nt - 1) / max_nt;
     // skinny problems (few 128-row m-tiles, e.g. the fully connected layers at batch 512) are latency-bound:
-    // trade operand re-reads for more CTAs by narrowing the n-tile until ~100 CTAs exist (measured: fc1 fwd 55 -> 45 us)
+    // trade operand re-reads for more CTAs by narrowing the n-tile until ~100 CTAs exist
     if (m_tiles_hint > 0) {
         while (m_tiles_hint * pl.n_tiles < 96 && (n_out + pl.n_tiles - 1) / pl.n_tiles > 48) pl.n_tiles *= 2;
     }
@@ -1683,18 +1618,17 @@ static Plan make_plan(int Cin_k, int KHW, int n_out, bool has_main, bool has_sig
     if (has_main) need = max(need, pl.main_col + pad_to(pl.n_t, 16));
     if (has_sigma) need = max(need, pl.sig_col + pad_to(pl.n_t, 16));
     if (has_wsum) need = max(need, pl.wsum_col + 16);
-    pl.tmem_cols = 32;
-    while (pl.tmem_cols < need) pl.tmem_cols <<= 1;
+    pl.acc_cols = need;
     const int stage_bytes = UM_A_STAGE + pl.n_mma * 128;
-    const int budget_kb = 100, max_stages = 4;          // 2 CTAs / SM; deeper rings per CTA measured slower than more CTAs
-    // kernels whose accumulators fit 128 TMEM columns (dgrad, narrow layers) run 3 CTAs/SM: more resident CTAs hide
-    // the load / barrier round-trip latency better than deeper per-CTA pipelines (measured: conv2 dgrad 144 -> 121 us)
-    const int budget = (pl.tmem_cols <= 128 && !has_sigma && budget_kb > 72) ? 72 : budget_kb;
-    pl.stages = (budget * 1024 - 2048) / stage_bytes;
+    const int max_stages = 4;                           // one CTA per SM (registers of the two MMA warpgroups)
+    pl.stages = (192 * 1024) / stage_bytes;
     if (pl.stages > max_stages) pl.stages = max_stages;
     if (pl.stages < 2) pl.stages = 2;
     if (pl.stages > pl.num_kb) pl.stages = pl.num_kb < 1 ? 1 : pl.num_kb;
-    pl.smem_bytes = 1024 + (size_t)pl.stages * stage_bytes + 16 * pl.stages + 64;
+    // the fp32 accumulator tile (128 rows, acc_cols + 4 floats apart) reuses the operand ring after the main loop
+    const int acc_bytes = UM_BLOCK_M * (pl.acc_cols + 4) * 4;
+    pl.ring_bytes = pad_to(max(pl.stages * stage_bytes, acc_bytes), 1024);
+    pl.smem_bytes = 1024 + (size_t)pl.ring_bytes + 16 * pl.stages + 64;
     pl.xp_bytes = (size_t)pixels_in * pl.Cp * 2;
     pl.wp_bytes = (size_t)pl.n_tiles * pl.num_kb * pl.n_mma * 64 * 2;
     return pl;
@@ -1718,7 +1652,7 @@ static bool make_shift_plan(const nn_conv_geom& g, bool noisy, ShiftPlan* out) {
     sp.main_col = 0;
     sp.sig_col = noisy ? sp.n_t : -1;
     sp.n_mma = pad_to(noisy ? 2 * sp.n_t : sp.n_t, 16);
-    if (sp.n_mma > SH_ACC_STRIDE) return false;
+    if (sp.n_mma > SH_MAX_N) return false;
     const int khw = g.KH * g.KW;
     sp.n_pairs = (khw + 1) / 2;
     sp.n_chunks = 2 * sp.n_pairs;
@@ -1729,10 +1663,10 @@ static bool make_shift_plan(const nn_conv_geom& g, bool noisy, ShiftPlan* out) {
     // (the A ring is sized for the block tiles of the pooled launches: 16 + KH - 1 image rows)
     const int a_stage_blk = pad_to(((15 + g.KH - 1) * g.W + 8 + (g.KW - 1) + 8) * 16, 128);
     sp.smem_bytes = 128 + (size_t)sp.b_bytes + (size_t)SH_STAGES * (a_stage_blk > sp.a_stage ? a_stage_blk : sp.a_stage) + 16 * SH_STAGES + 64 +
-                    4 * SH_MAX_PAIRS + 16 + 12 * 1024;
+                    4 * SH_MAX_PAIRS + 16 + 12 * 1024 + (size_t)UM_BLOCK_M * (sp.n_mma + 4) * 4;
     if (sp.n_pairs > SH_MAX_PAIRS) return false;
     sp.wp_bytes = (size_t)sp.b_bytes;
-    if (sp.smem_bytes > 200 * 1024) return false;
+    if (sp.smem_bytes > 227 * 1024) return false;
     if (out) *out = sp;
     return true;
 }
@@ -1741,7 +1675,7 @@ static bool make_shift_plan(const nn_conv_geom& g, bool noisy, ShiftPlan* out) {
 long long* g_dbg_buf = nullptr;
 size_t g_dbg_ctas = 0, g_dbg_last = 0;
 
-// measurement hook: CUDA events around the main tcgen05 kernel only (excludes the operand packs)
+// measurement hook: CUDA events around the main tensor-core kernel only (excludes the operand packs)
 int g_time_main = 0;
 cudaEvent_t g_ev0 = nullptr, g_ev1 = nullptr;
 
@@ -1753,17 +1687,17 @@ static int nn_num_sms_cached() {
 
 static int launch_umma(const UmmaP& p, const Plan& pl, cudaStream_t st, void* splitk_ws = nullptr, size_t splitk_ws_bytes = 0) {
     NN_ONCE_PER_DEVICE({
-        NN_CUDA_OK(cudaFuncSetAttribute(k_conv_umma<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        NN_CUDA_OK(cudaFuncSetAttribute(k_conv_umma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        NN_CUDA_OK(cudaFuncSetAttribute(k_conv_umma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        NN_CUDA_OK(cudaFuncSetAttribute(k_conv_umma<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        NN_CUDA_OK(cudaFuncSetAttribute(k_conv_umma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        NN_CUDA_OK(cudaFuncSetAttribute(k_conv_umma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     });
     const bool extras = p.bias || p.mask_x || p.z_inject || p.z_export || p.sigma_export || p.stats;
     int epi = 0;
     if (!extras && p.main_col >= 0 && p.noise_mode != NN_NOISE_NONE && p.y_noisy) epi = 1;
     else if (!extras && p.main_col >= 0 && p.noise_mode == NN_NOISE_NONE && p.y) epi = 2;
     UmmaP pd = p;
-    // measured at batch 512 (same run, A/B): incremental tap tracking takes conv2 dgrad 120 -> 110 us (3 CTAs/SM, the
-    // producers' issue slots matter) but costs the fused forward 70 -> 72.7 us (2 CTAs/SM, sigma rows): per variant
+    // incremental tap tracking saves the producers' divisions on the plain (dgrad) variant; the noisy forward keeps the
+    // direct computation
     pd.inc_taps = epi == 2 ? 1 : 0;
     pd.rows_tile = UM_BLOCK_M;
     dim3 grid((p.M + pd.rows_tile - 1) / pd.rows_tile, pl.n_tiles);
@@ -1785,7 +1719,7 @@ static int launch_umma(const UmmaP& p, const Plan& pl, cudaStream_t st, void* sp
 #endif
     // split-K for skinny linear layers (few m-tiles x n-tiles, long K: fc1 forward at batch 512 is 52 CTAs walking 47
     // k-blocks each -- a latency chain on a third of the SMs): the k-blocks are dealt to gridDim.z CTAs that dump raw
-    // accumulators, and k_splitk_epilogue sums them and applies the noise epilogue (measured: 1: 0.805, 3: 0.788, 4: 0.785 ms/step)
+    // accumulators, and k_splitk_epilogue sums them and applies the noise epilogue
     int splits = 1;
     if ((epi == 1 || epi == 2) && p.OH * p.OW == 1 && !want_dbg && (int)(grid.x * grid.y) * 2 <= nn_num_sms_cached() && pl.num_kb >= 8 && splitk_ws) {
         splits = 4;
@@ -2024,13 +1958,13 @@ static int shift_conv_fwd(const nn_conv_fwd_args* a, const ShiftPlan& sp, int de
         if (!g_ev0) { cudaEventCreate(&g_ev0); cudaEventCreate(&g_ev1); }
         cudaEventRecord(g_ev0, st);
     }
-    const int mode = !noise ? 0 : (a->z_inject ? 2 : 1);      // 16 epilogue warps (12 / 20 / 24 measured slower)
+    const int mode = !noise ? 0 : (a->z_inject ? 2 : 1);      // 16 epilogue warps
 #define NN_SHIFT_LAUNCH(MODE, EW, POOL)                                                                                \
     do {                                                                                                               \
         NN_ONCE_PER_DEVICE({ \
-            NN_CUDA_OK(cudaFuncSetAttribute(k_conv_shift<MODE, EW, POOL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
+            NN_CUDA_OK(cudaFuncSetAttribute(k_conv_shift<MODE, EW, POOL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
         });                                                                                                              \
-        k_conv_shift<MODE, EW, POOL><<<grid, (2 + EW) * 32, sp.smem_bytes, st>>>(p);                                    \
+        k_conv_shift<MODE, EW, POOL><<<grid, (1 + EW) * 32, sp.smem_bytes, st>>>(p);                                    \
     } while (0)
     if (p.pooled) {
         if (mode == 0) NN_SHIFT_LAUNCH(0, 16, true); else if (mode == 1) NN_SHIFT_LAUNCH(1, 16, true); else NN_SHIFT_LAUNCH(2, 16, true);
@@ -2157,7 +2091,7 @@ static int tma_conv_fwd(const nn_conv_fwd_args* a, const TmaPlan& tp, int device
 
 int nn_umma_conv_fwd(const nn_conv_fwd_args* a, int device, cudaStream_t st) {
     if (a->precision != NN_PREC_BF16)
-        return nn_fail("nn_noisy_conv_fwd: tcgen05 path implements NN_PREC_BF16 only%s", "");
+        return nn_fail("nn_noisy_conv_fwd: tensor-core path implements NN_PREC_BF16 only%s", "");
     const nn_conv_geom& g = a->g;
     int OH, OW;
     nn_out_hw(g, OH, OW);
@@ -2227,7 +2161,7 @@ int nn_umma_conv_fwd(const nn_conv_fwd_args* a, int device, cudaStream_t st) {
     memset(&p, 0, sizeof(p));
     p.B = g.B; p.H = g.H; p.W = g.W; p.Cp = pl.Cp; p.KH = g.KH; p.KW = g.KW; p.stride = g.stride; p.pad = g.pad;
     p.OH = OH; p.OW = OW; p.M = g.B * OH * OW; p.Cout = g.Cout; p.n_t = pl.n_t; p.n_mma = pl.n_mma;
-    p.num_kb = pl.num_kb; p.stages = pl.stages; p.tmem_cols = pl.tmem_cols;
+    p.num_kb = pl.num_kb; p.stages = pl.stages; p.acc_cols = pl.acc_cols; p.ring_bytes = pl.ring_bytes;
     p.main_col = pl.main_col; p.sig_col = pl.sig_col; p.wsum_col = pl.wsum_col;
     p.xp = xp; p.wp = wp;
     const float as = a->a_code_scale > 0.f ? a->a_code_scale : 1.f;
@@ -2364,7 +2298,7 @@ extern "C" int nn_prepare_weights(const nn_wprep_job* jobs, int count, int devic
 
 int nn_umma_conv_dgrad(const nn_conv_dgrad_args* a, int device, cudaStream_t st) {
     if (a->precision != NN_PREC_BF16)
-        return nn_fail("nn_noisy_conv_dgrad: tcgen05 path implements NN_PREC_BF16 only%s", "");
+        return nn_fail("nn_noisy_conv_dgrad: tensor-core path implements NN_PREC_BF16 only%s", "");
     const nn_conv_geom& g = a->g;
     int OH, OW;
     nn_out_hw(g, OH, OW);
@@ -2452,20 +2386,20 @@ int nn_umma_conv_dgrad(const nn_conv_dgrad_args* a, int device, cudaStream_t st)
     memset(&p, 0, sizeof(p));
     p.B = g.B; p.H = OH; p.W = OW; p.Cp = pl.Cp; p.KH = g.KH; p.KW = g.KW; p.stride = 1; p.pad = g.KH - 1 - g.pad;
     p.OH = g.H; p.OW = g.W; p.M = g.B * g.H * g.W; p.Cout = g.Cin; p.n_t = pl.n_t; p.n_mma = pl.n_mma;
-    p.num_kb = pl.num_kb; p.stages = pl.stages; p.tmem_cols = pl.tmem_cols;
+    p.num_kb = pl.num_kb; p.stages = pl.stages; p.acc_cols = pl.acc_cols; p.ring_bytes = pl.ring_bytes;
     p.main_col = pl.main_col; p.sig_col = -1; p.wsum_col = -1;
     p.xp = xp; p.wp = wp; p.y_scale = a->w_code_scale > 0.f ? a->w_code_scale : 1.f; p.s_scale = 1.f;
     p.y = a->gx; p.noise_mode = NN_NOISE_NONE;
     p.mask_x = a->x_pre; p.mask_lo = (float)a->x_lo; p.mask_hi = (float)a->x_hi;
     p.err_flag = nn_umma_err_flag(device);
     if (g.KH != g.KW && (g.KH - 1 - g.pad) != (g.KW - 1 - g.pad))
-        return nn_fail("nn_noisy_conv_dgrad: non-square kernels not supported on the tcgen05 path%s", "");
+        return nn_fail("nn_noisy_conv_dgrad: non-square kernels not supported on the tensor-core path%s", "");
     return launch_umma(p, pl, st);
 }
 
 namespace {
 struct WgPlan {
-    int Cp, Coutp, Ktot, n_tiles_k, NT, ktot_pad, m_tiles_n, num_kb, splits, kb_per_split, stages, tmem_cols;
+    int Cp, Coutp, Ktot, n_tiles_k, NT, ktot_pad, m_tiles_n, num_kb, splits, kb_per_split, stages;
     size_t xp_bytes, gyp_bytes, partial_bytes, smem_bytes;
 };
 WgPlan make_wg_plan(const nn_conv_geom& g, int device) {
@@ -2483,17 +2417,15 @@ WgPlan make_wg_plan(const nn_conv_geom& g, int device) {
     w.m_tiles_n = (g.Cout + 127) / 128;
     w.num_kb = (int)((Mpix + 63) / 64);
     const int tiles = w.n_tiles_k * w.m_tiles_n;
-    int splits = (2 * nn_num_sms(device) + tiles - 1) / tiles;
+    int splits = (nn_num_sms(device) + tiles - 1) / tiles;
     if (splits > w.num_kb) splits = w.num_kb;
     if (splits < 1) splits = 1;
     w.kb_per_split = (w.num_kb + splits - 1) / splits;
     w.splits = (w.num_kb + w.kb_per_split - 1) / w.kb_per_split;
     const int stage_bytes = UM_A_STAGE + w.NT * 128;
-    w.stages = (100 * 1024 - 3072) / stage_bytes;
+    w.stages = (192 * 1024) / stage_bytes;
     if (w.stages > 4) w.stages = 4;
     if (w.stages < 2) w.stages = 2;
-    w.tmem_cols = 32;
-    while (w.tmem_cols < w.NT) w.tmem_cols <<= 1;
     w.smem_bytes = 1024 + (size_t)w.stages * stage_bytes + 16 * w.stages + 64 + (size_t)(w.NT / 8) * 16 + 16;
     w.xp_bytes = (size_t)g.B * g.H * g.W * w.Cp * 2;
     w.gyp_bytes = (size_t)Mpix * w.Coutp * 2;
@@ -2506,7 +2438,7 @@ WgPlan make_wg_plan(const nn_conv_geom& g, int device) {
 
 namespace {
 struct WgShiftPlan {
-    int n_planes, n_row, n_chunks, b_pixels, a_stage, b_stage, stages, tmem_cols, grid;
+    int n_planes, n_row, n_chunks, b_pixels, a_stage, b_stage, stages, grid;
     int64_t plane_stride;
     size_t smem_bytes, xp_bytes, gyv_bytes, partial_bytes;
 };
@@ -2516,10 +2448,7 @@ bool make_wg_shift_plan(const nn_conv_geom& g, int device, WgShiftPlan* out) {
     WgShiftPlan w;
     w.n_planes = (g.Cout + 7) / 8;
     w.n_row = pad_to(g.KW * 8, 16);
-    const int need = g.KH * w.n_row;
-    if (need > 512 || w.n_row > 256) return false;
-    w.tmem_cols = 32;
-    while (w.tmem_cols < need) w.tmem_cols <<= 1;
+    if (w.n_row > 64) return false;                     // k_wgrad_shift<16 / 32 / 48 / 64>
     const int64_t total = (int64_t)g.B * g.H * g.W;
     w.plane_stride = (total + WS_KP - 1) / WS_KP * WS_KP;
     w.n_chunks = (int)(w.plane_stride / WS_KP);
@@ -2527,15 +2456,11 @@ bool make_wg_shift_plan(const nn_conv_geom& g, int device, WgShiftPlan* out) {
     w.a_stage = w.n_planes * WS_KP * 16;
     w.b_stage = pad_to(w.b_pixels * 16, 128);
     const int fixed = 128 + 16 * WS_KP * 16 + 16 * WS_MAX_STAGES + 64;
-    // two CTAs per SM when the accumulators leave room in TMEM: one CTA's MMA stream has issue gaps (barrier waits,
-    // commits, accumulator switches) that a second stream fills -- measured at batch 512: CTA span 70 -> 35 us
-    const int env_ctas = 2;
-    const int ctas = (env_ctas == 2 && w.tmem_cols <= 256) ? 2 : 1;
-    w.stages = ((ctas == 2 ? 100 : 190) * 1024 - fixed) / (w.a_stage + w.b_stage);
+    w.stages = (190 * 1024 - fixed) / (w.a_stage + w.b_stage);         // one CTA per SM (accumulator registers)
     if (w.stages > WS_MAX_STAGES) w.stages = WS_MAX_STAGES;
     if (w.stages < 2) return false;
     w.smem_bytes = (size_t)fixed + (size_t)w.stages * (w.a_stage + w.b_stage);
-    w.grid = ctas * nn_num_sms(device);
+    w.grid = nn_num_sms(device);
     if (w.grid > w.n_chunks) w.grid = w.n_chunks;
     w.xp_bytes = (size_t)total * 16;
     w.gyv_bytes = (size_t)w.n_planes * w.plane_stride * 16;
@@ -2615,13 +2540,14 @@ static int shift_conv_wgrad(const nn_conv_wgrad_args* a, const WgShiftPlan& w, i
     memset(&p, 0, sizeof(p));
     p.H = g.H; p.W = g.W; p.OH = OH; p.OW = OW; p.KH = g.KH; p.KW = g.KW; p.Cout = g.Cout;
     p.n_planes = w.n_planes; p.n_row = w.n_row; p.n_chunks = w.n_chunks; p.b_pixels = w.b_pixels;
-    p.a_stage = w.a_stage; p.b_stage = w.b_stage; p.stages = w.stages; p.tmem_cols = w.tmem_cols;
+    p.a_stage = w.a_stage; p.b_stage = w.b_stage; p.stages = w.stages;
     p.total_pixels = (long long)g.B * g.H * g.W; p.plane_stride = w.plane_stride;
-    const int env_order = 1;      // kernel row outermost (8 MMAs per accumulator in a row)
-    p.order = env_order;
     p.xp = xp; p.gyv = gyv; p.partial = partial; p.err_flag = nn_umma_err_flag(device);
     NN_ONCE_PER_DEVICE({
-        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_shift, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_shift<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_shift<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_shift<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_shift<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     });
 #ifdef NN_KDEBUG
     static const bool want_dbg = getenv("NN_UMMA_DEBUG") != nullptr;
@@ -2641,7 +2567,10 @@ static int shift_conv_wgrad(const nn_conv_wgrad_args* a, const WgShiftPlan& w, i
     }
     const int kcols = g.KH * g.KW * 8;
     p.row_pitch = kcols <= 256 ? 256 : kcols;
-    k_wgrad_shift<<<w.grid, WS_THREADS, w.smem_bytes, st>>>(p);
+    if (w.n_row == 16) k_wgrad_shift<16><<<w.grid, WS_THREADS, w.smem_bytes, st>>>(p);
+    else if (w.n_row == 32) k_wgrad_shift<32><<<w.grid, WS_THREADS, w.smem_bytes, st>>>(p);
+    else if (w.n_row == 48) k_wgrad_shift<48><<<w.grid, WS_THREADS, w.smem_bytes, st>>>(p);
+    else k_wgrad_shift<64><<<w.grid, WS_THREADS, w.smem_bytes, st>>>(p);
     NN_LAUNCH_OK();
     const float scale = a->a_code_scale > 0.f ? a->a_code_scale : 1.f;
     if (kcols <= 256) {
@@ -2671,7 +2600,7 @@ static int shift_conv_wgrad(const nn_conv_wgrad_args* a, const WgShiftPlan& w, i
 
 int nn_umma_conv_wgrad(const nn_conv_wgrad_args* a, int device, cudaStream_t st) {
     if (a->precision != NN_PREC_BF16)
-        return nn_fail("nn_noisy_conv_wgrad: tcgen05 path implements NN_PREC_BF16 only%s", "");
+        return nn_fail("nn_noisy_conv_wgrad: tensor-core path implements NN_PREC_BF16 only%s", "");
     const nn_conv_geom& g = a->g;
     int OH, OW;
     nn_out_hw(g, OH, OW);
@@ -2726,7 +2655,7 @@ int nn_umma_conv_wgrad(const nn_conv_wgrad_args* a, int device, cudaStream_t st)
         memset(&r, 0, sizeof(r));
         r.main = partial;
         r.tail = tw.tail_w ? reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(partial) + tw.main_bytes) : nullptr;
-        r.splits = tw.splits; r.n_tail = tw.splits * tw.tiles_k; r.Cout = g.Cout; r.Cin = g.Cin; r.KHW = g.KH * g.KW; r.n_c64 = tw.n_c64;
+        r.splits = tw.splits; r.n_tail = tw.splits; r.Cout = g.Cout; r.Cin = g.Cin; r.KHW = g.KH * g.KW; r.n_c64 = tw.n_c64;
         r.cols_pad = tw.cols_pad; r.scale = scale; r.lo = (float)a->w_lo; r.hi = (float)a->w_hi; r.gw = a->gw; r.w_raw = a->w_raw;
         auto groups = [](int64_t quads, int cnt) {      // ~128 k threads, at least ~4 partials per thread
             int G = 1;
@@ -2747,10 +2676,10 @@ int nn_umma_conv_wgrad(const nn_conv_wgrad_args* a, int device, cudaStream_t st)
     p.B = g.B; p.H = g.H; p.W = g.W; p.Cp = w.Cp; p.KH = g.KH; p.KW = g.KW; p.stride = g.stride; p.pad = g.pad;
     p.OH = OH; p.OW = OW; p.Mpix = g.B * OH * OW; p.Cout = g.Cout; p.Coutp = w.Coutp;
     p.Ktot = w.Ktot; p.NT = w.NT; p.ktot_pad = w.ktot_pad; p.num_kb = w.num_kb; p.kb_per_split = w.kb_per_split;
-    p.stages = w.stages; p.tmem_cols = w.tmem_cols; p.xp = xp; p.gyp = gyp; p.partial = partial;
+    p.stages = w.stages; p.xp = xp; p.gyp = gyp; p.partial = partial;
     p.err_flag = nn_umma_err_flag(device);
     NN_ONCE_PER_DEVICE({
-        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_umma, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_umma, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     });
     dim3 grid(w.n_tiles_k, w.m_tiles_n, w.splits);
     k_wgrad_umma<<<grid, UM_THREADS, w.smem_bytes, st>>>(p);

@@ -17,7 +17,7 @@ extern "C" int nn_device_info(int device, int* sm_count, int* cc_major, int* cc_
     if (sm_count) *sm_count = sms;
     if (cc_major) *cc_major = maj;
     if (cc_minor) *cc_minor = min_;
-    if (maj != 10) return nn_fail("noisynet_b200 is built for sm_100a only; device has compute capability %s%lld", "", (long long)maj);
+    if (maj != 9 || min_ != 0) return nn_fail("noisynet_b200 is built for sm_90a only; device has compute capability %s%lld", "", (long long)(10 * maj + min_));
     return 0;
 }
 

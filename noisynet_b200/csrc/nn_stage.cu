@@ -21,7 +21,7 @@ namespace {
 constexpr int ST_SPLITS = 16;   // MAX batch slices per channel for the deterministic partial sums (gridDim.y <= ST_SPLITS)
 
 // slices actually used: enough blocks to fill the GPU, but at least ~2048 elements per block (the fc stages have 512
-// elements per channel: 16 slices of 32 elements were pure launch overhead, 10 us for a 0.8 MB tensor)
+// elements per channel: 16 slices of 32 elements are pure launch overhead)
 static inline int stage_splits(int64_t per_channel) {
     int64_t s = per_channel / 2048;
     if (s < 1) s = 1;
@@ -783,7 +783,7 @@ k_head_rows(const float* __restrict__ z, const int64_t* __restrict__ label, int 
 // ------------------------------------------------------------------ classifier tail, fused (noisynet.py:589-594, :1278)
 // fc2 forward with its current noise -> BatchNorm1d (batch statistics) -> mean cross entropy -> gradient back
 // through both -> fc2 dgrad, for a layer with <= 16 output units: three launches of a few microseconds of work each
-// sat back to back on the critical path of the step (tcgen05 forward 11 us, head 18 us, tcgen05 dgrad 9 us).
+// sat back to back on the critical path of the step (tensor-core forward, head, tensor-core dgrad).
 // ONE thread-block cluster of 8 CTAs: each CTA owns B/8 samples, keeps its activation rows (bf16 codes) and the
 // whole weight matrix (codes + g(|w|)) in shared memory, and the two batch-wide reductions (BN statistics; dbeta /
 // dgamma / loss) go through distributed shared memory with a cluster barrier -- fixed summation order, identical in
@@ -1267,7 +1267,7 @@ extern "C" int nn_input_gather_quant_pack(const float* data, const int64_t* idx,
 // Hot path of the first layer's input (C <= 4 channels in ONE 8-channel chunk, k-bit codes, Philox stochastic rounding, no
 // fp32 copy): a thread owns FOUR consecutive pixels -- one float4 load per channel, four 16-byte code stores = 64 contiguous
 // bytes -- so every thread has all its loads in flight at once (the one-item-per-trip kernel above ran two latency-bound
-// rounds: 14 us for 14 MB).  Same Philox counter per pixel and the same arithmetic: bit-identical codes.
+// rounds).  Same Philox counter per pixel and the same arithmetic: bit-identical codes.
 __global__ void __launch_bounds__(256)
 k_quant_pack_input4(const float* __restrict__ x, __nv_bfloat16* __restrict__ xp, int B, int C, int HW, float q_scale, float q_max,
                     float stoch, nn_rng rng) {

@@ -1,9 +1,9 @@
 """NoisyNetEngine -- the whole CIFAR NoisyNet training step (noisynet.py:1276-1542) as an explicit schedule
 of this library's kernels, with static buffers (CUDA-graph capturable, no autograd, no torch kernels):
 
-  forward : input quantize+pack -> [tcgen05 fused noisy conv -> pool+BN+ReLU+clamp+quantize+pack stage] x 2
-            -> [tcgen05 fused noisy linear -> BN+ReLU+clamp+quantize+pack stage] -> fused noisy linear -> BN + CE head
-  backward: head -> wgrad/dgrad (tcgen05) -> stage backward (STE/clamp/ReLU masks, BN backward, pool routing,
+  forward : input quantize+pack -> [tensor-core fused noisy conv -> pool+BN+ReLU+clamp+quantize+pack stage] x 2
+            -> [tensor-core fused noisy linear -> BN+ReLU+clamp+quantize+pack stage] -> fused noisy linear -> BN + CE head
+  backward: head -> wgrad/dgrad (tensor cores) -> stage backward (STE/clamp/ReLU masks, BN backward, pool routing,
             emitted as NHWC bf16 for the next wgrad/dgrad) ... -> conv1 wgrad
   update  : [flat-gradient all-reduce] -> fused AdamW + weight clamp + max|W|
 
@@ -107,11 +107,10 @@ class NoisyNetEngine:
         # conv1 weight gradient through the in-place (shift) kernel: its grad_output lives in the planes layout on the
         # 32x32 input grid, zeroed once here -- nn_stage_bwd only ever writes the 28x28 output positions
         # MaxPool2d and the batch statistics of bn1 fused into the conv1 epilogue (pooled_out + bn_mean): exact, the 104 MB y1n
-        # round trip and the pool+statistics pass (33 us) disappear; conv1 forward 78 -> 97 us on block tiles whose 2x2
-        # windows lie inside one warp (round 1's per-group pair barrier made it 123 us).  NN_ENGINE_FUSE_POOL=0: separate stage
-        # fc2 + bn4 + loss + their backward as ONE 8-CTA cluster launch (nn_classifier_tail): exact and tested, but 43 us
-        # against 37 us for the three separate launches it replaces (8 SMs, ten latency-bound phases) -- off unless
-        # NN_ENGINE_FUSED_TAIL=1
+        # round trip and the pool+statistics pass disappear; the conv1 forward runs on block tiles whose 2x2 windows lie
+        # inside one warp.  NN_ENGINE_FUSE_POOL=0: separate stage
+        # fc2 + bn4 + loss + their backward as ONE 8-CTA cluster launch (nn_classifier_tail): exact and tested, but it runs
+        # ten latency-bound phases on 8 SMs instead of three short launches -- off unless NN_ENGINE_FUSED_TAIL=1
         self.fused_tail = B <= 2048 and self.q_w[3] > 0 and self.q_a[3] > 0 and os.environ.get("NN_ENGINE_FUSED_TAIL", "0") == "1"
         self.fuse_pool1 = bool(self.lib.nn_conv_pool_fusable(C.byref(self.geom[0]), self.noise_modes[0], PREC_BF16)) and \
             os.environ.get("NN_ENGINE_FUSE_POOL", "1") == "1"
@@ -397,7 +396,7 @@ class NoisyNetEngine:
         if self.side is not None:
             # conv1's image is needed at once; the other six (fc1 is 90 % of the bytes) are packed on the side stream
             # while the input pack and the conv1 forward run, and joined before conv2.  (Moving the input pack to the side
-            # stream as well, next to conv1's image, measured 30 us SLOWER per step: it delays the six images.)
+            # stream as well, next to conv1's image, would delay the six images.)
             self.side.wait_stream(torch.cuda.current_stream(di))
             with torch.cuda.stream(self.side):
                 _lib.check(lib.nn_prepare_weights(C.byref(self.jobs[1]), 6, di, self._st()), "nn_prepare_weights")

@@ -1,7 +1,7 @@
 """Drop-in replacement for the reference's ``hardware_model`` module (hardware_model.py).
 
 Same names, signatures, state_dict keys and error behaviour; every arithmetic op runs in the
-sm_100a kernels behind the C ABI (include/noisynet_b200.h).  Put ``<repo>/dropin`` ahead of the
+sm_90a kernels behind the C ABI (include/noisynet_b200.h).  Put ``<repo>/dropin`` ahead of the
 reference on ``sys.path`` and ``noisynet.py`` / ``models/resnet.py`` / ``main.py`` import this
 instead (noisynet.py:14, models/resnet.py:11, main.py:37).
 
@@ -186,7 +186,7 @@ def _f32(v):
 
 
 def code_scales(x, w):
-    """Integer-code scales for the tcgen05 path from the tags QuantMeasure / _prepare_weight leave on their
+    """Integer-code scales for the tensor-core path from the tags QuantMeasure / _prepare_weight leave on their
     outputs: activations on the grid k * s (min 0) -> a_code_scale = s; weights on a symmetric grid
     (2k - qmax) * s/2 -> w_code_scale = s/2.  0.0 = no exact code representation."""
     a_cs = w_cs = 0.0

@@ -98,7 +98,7 @@ class NoisyNet(nn.Module):
             return y
         # ---- fused: one launch
         weight, bias, ste = _prepare_weight(mod, linear=(kind == "linear"))
-        a_cs, w_cs = code_scales(x, weight)          # exact integer operands on the tcgen05 path
+        a_cs, w_cs = code_scales(x, weight)          # exact integer operands on the tensor-core path
         w_raw = mod.weight.detach()
         if kind == "linear":
             x4 = x.reshape(x.shape[0], -1, 1, 1)

@@ -15,7 +15,7 @@ from ._lib import (NOISE_EXTERNAL, NOISE_MERGED, NOISE_NONE, PREC_BF16, PREC_FP3
                    ConvDgradArgs, ConvFwdArgs, ConvGeom, ConvWgradArgs, Rng)
 
 # Default arithmetic of the contraction kernels.  PREC_FP32 = CUDA-core fp32 (reference arithmetic);
-# PREC_BF16 = tcgen05 (exact for integer codes, bf16-rounded operands otherwise).  Overridable per call or globally.
+# PREC_BF16 = tensor cores (exact for integer codes, bf16-rounded operands otherwise).  Overridable per call or globally.
 # "tf32" is declared in the C ABI but not implemented: asking for it raises instead of silently running something else.
 _default_precision = PREC_FP32
 _PREC_NAMES = {"fp32": PREC_FP32, "bf16": PREC_BF16}
@@ -23,7 +23,7 @@ _PREC_NAMES = {"fp32": PREC_FP32, "bf16": PREC_BF16}
 
 def _prec_by_name(p):
     if p == "tf32" or p == PREC_TF32:
-        raise ValueError("noisynet_b200: precision 'tf32' is not implemented; use 'bf16' (tcgen05, bf16-rounded operands, "
+        raise ValueError("noisynet_b200: precision 'tf32' is not implemented; use 'bf16' (tensor cores, bf16-rounded operands, "
                          "fp32 accumulate, 1.5e-2 tolerance) or 'fp32' (CUDA cores)")
     return _PREC_NAMES[p]
 
@@ -289,14 +289,14 @@ def alt_noise(y, kind, level, rnd=None, rng=None):
 
 
 def _pick_prec(prec, g, which):
-    """tcgen05 precisions serve a subset of geometries; the rest run on the fp32 CUDA-core kernels."""
+    """tensor-core precisions serve a subset of geometries; the rest run on the fp32 CUDA-core kernels."""
     if prec != PREC_FP32 and not _lib.load().nn_conv_supported(C.byref(g), int(prec), which):
         return PREC_FP32
     return prec
 
 
 def error_flag(dev=0, reset=True):
-    """Synchronises and returns the tcgen05 pipeline watchdog flag (0 = ok)."""
+    """Synchronises and returns the tensor-core pipeline watchdog flag (0 = ok)."""
     return _lib.load().nn_debug_error_flag(int(dev), 1 if reset else 0)
 
 

@@ -1,9 +1,9 @@
 """Mint golden fixtures by running the UNMODIFIED reference modules (CPU, shimmed).
 
-Run in the build container only (needs /root/reference):
-    python -m oracle.gen_golden
-Writes small .npz files under tests/golden/.  The reference cannot travel to the GPU box,
-the fixtures do.  Every case stores the inputs, the random tensors the reference consumed
+Needs a checkout of the reference (michaelklachko/NoisyNet) named by NOISYNET_REFERENCE:
+    NOISYNET_REFERENCE=<checkout> python -m oracle.gen_golden
+Writes small .npz files under tests/golden/.  The tests read only those fixtures, never the
+reference itself.  Every case stores the inputs, the random tensors the reference consumed
 (recovered by re-seeding the generator) and the reference's outputs.
 """
 import os

@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """Mints tests/golden/script_trace.npz: the loss curve of the UNMODIFIED reference script
-(/root/reference/noisynet.py, module-level training loop :1215-1542) over its first steps, on a deterministic
-synthetic dataset -- the fixture the GPU test of the drop-in modules compares against (the reference tree does not
-exist on the GPU box, SURVEY 8c).  Test infrastructure; run in the build container only:
+(noisynet.py, module-level training loop :1215-1542) over its first steps, on a deterministic synthetic dataset --
+the fixture the GPU test of the drop-in modules compares against (the tests never read the reference itself).
+Needs a checkout of the reference (michaelklachko/NoisyNet) named by NOISYNET_REFERENCE:
 
-    python oracle/gen_script_trace.py            # CPU, ~2 min
+    NOISYNET_REFERENCE=<checkout> python oracle/gen_script_trace.py            # CPU, a few minutes
 
 Process-level shims only (SURVEY Appendix A): matplotlib / torch._six stubs, .cuda() -> identity, distribution
 validation off, np.random seeded (the script seeds `random` and torch but permutes with np.random, noisynet.py:1232),
@@ -19,7 +19,7 @@ import textwrap
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get("NOISYNET_REFERENCE", "/root/reference")
+REF = os.environ.get("NOISYNET_REFERENCE", "")
 
 STEPS = 60
 BATCH = 64

@@ -1,7 +1,7 @@
 """CPU restatement (torch-CPU fp32 + numpy) of the NoisyNet hot path.
 
 TEST INFRASTRUCTURE ONLY -- see ``oracle/__init__.py``.  Every function cites
-the reference lines (``/root/reference``, commit 34b7996) it restates.  The
+the reference lines (michaelklachko/NoisyNet, commit 34b7996) it restates.  The
 arithmetic of the reference lives in PyTorch (ATen, fp32); this file therefore
 uses torch CPU fp32 ops for the contractions and restates everything the
 reference writes itself (quantizer, STE, weight noise, current noise, side

@@ -1,8 +1,8 @@
 """Process-level shims that let the UNMODIFIED reference import and run on CPU.
 
-Only usable where ``/root/reference`` exists (the build container); used by
-``oracle/gen_golden.py`` to mint the golden fixtures and by optional
-oracle-vs-reference tests.  Never imported by the product package.
+Only usable next to a checkout of the reference (michaelklachko/NoisyNet), named by the environment
+variable NOISYNET_REFERENCE; used by ``oracle/gen_golden.py`` to mint the golden fixtures under
+tests/golden/.  Never imported by the product package or the tests.
 
 Shims (SURVEY §8c): (1) matplotlib stub (hardware_model.py:9 -> plot_histograms.py:1-4),
 (2) torch._six stub (models/conv2d_layers.py:4), (3) .cuda() -> identity on GPU-less hosts
@@ -16,7 +16,7 @@ import types
 
 import torch
 
-REFERENCE_ROOT = os.environ.get("NOISYNET_REFERENCE", "/root/reference")
+REFERENCE_ROOT = os.environ.get("NOISYNET_REFERENCE", "")
 
 
 def reference_available():
@@ -25,7 +25,8 @@ def reference_available():
 
 def install():
     if not reference_available():
-        raise RuntimeError("reference tree not found at %s" % REFERENCE_ROOT)
+        raise RuntimeError("reference tree not found at %r: set NOISYNET_REFERENCE to a checkout of michaelklachko/NoisyNet"
+                           % REFERENCE_ROOT)
     if REFERENCE_ROOT not in sys.path:
         sys.path.insert(0, REFERENCE_ROOT)
     if "matplotlib" not in sys.modules:

@@ -4,7 +4,7 @@ exactly as models/resnet.py:16-62 builds it -- quantize1 -> conv1 3x3 (stride s,
 models/resnet.py:72-155) -- against the same block evaluated on the CPU with the oracle's functions.
 
 Deterministic configuration (stochastic rounding off, weight noise off, fixed activation ranges) so that the only
-differences are arithmetic: fp32 kernels within 2e-5 relative of the oracle; tcgen05 kernels exact for the 4-bit
+differences are arithmetic: fp32 kernels within 2e-5 relative of the oracle; tensor-core kernels exact for the 4-bit
 forward contractions (integer codes) and within the bf16 operand tolerance (1.5e-2 of max) for the gradients.
 Geometries exercised through the public module API: 3x3 pad 1 stride 1/2, 1x1 stride 2, 16 -> 32 channels.
 """

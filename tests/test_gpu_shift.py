@@ -1,5 +1,5 @@
 """The persistent shift-GEMM forward (k_conv_shift: narrow-input layers, weights resident in shared memory, the
-im2col rows read through shifted SWIZZLE_NONE descriptors) against the tiled tcgen05 kernel, the fp32 CUDA-core
+im2col rows read through shifted SWIZZLE_NONE descriptors) against the tiled tensor-core kernel, the fp32 CUDA-core
 kernel and a float64 evaluation.
 
 Stated tolerances (same as test_gpu_umma.py): integer-code main contraction exact up to the final scale multiply
@@ -119,7 +119,7 @@ WG_SHAPES = [  # B, Cin, H, W, Cout, k
 def test_shift_wgrad_matches_tiled_and_fp64(dev, shape):
     """Weight gradient through the in-place (shift) kernel: integer activation codes x bf16 grad_output, fp32
     accumulation.  Against float64 on the SAME bf16-rounded grad_output the only error is the fp32 summation
-    (rtol 2e-5 of the largest entry); against the tiled tcgen05 kernel (same operands, different summation order)
+    (rtol 2e-5 of the largest entry); against the tiled tensor-core kernel (same operands, different summation order)
     likewise."""
     from noisynet_b200 import _lib, ops
     from noisynet_b200._lib import PACK_SHIFT, PREC_BF16, ConvGeom

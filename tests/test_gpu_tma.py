@@ -1,5 +1,5 @@
 """The persistent CTA-pair kernel with TMA-im2col operands (csrc/nn_conv_tma.cu) against float64 evaluations of the same
-operands, the fp32 CUDA-core kernels and the gathered-im2col tcgen05 kernel it replaces on the lean path.
+operands, the fp32 CUDA-core kernels and the gathered-im2col tensor-core kernel it replaces on the lean path.
 
 Stated tolerances (as in test_gpu_umma.py):
   * integer-code mode: the tensor-core sum is exact -> rtol 1e-6 against float64;

@@ -1,4 +1,4 @@
-"""tcgen05 (NN_PREC_BF16) kernels against the fp32 CUDA-core kernels / the CPU oracle.
+"""Tensor-core (NN_PREC_BF16) kernels against the fp32 CUDA-core kernels / the CPU oracle.
 
 Stated tolerances:
   * integer-code mode (4-bit activation codes x odd-integer weight codes): the tensor-core sum is EXACT

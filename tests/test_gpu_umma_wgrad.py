@@ -1,4 +1,4 @@
-"""tcgen05 wgrad (MN-major operands, split reduction) against torch's fp32 conv2d_weight.
+"""Tensor-core wgrad (MN-major operands, split reduction) against torch's fp32 conv2d_weight.
 Tolerance: grad_output (and, outside code mode, the activations) are rounded to bf16 before the
 tensor-core contraction -> |err| <= 1.5e-2 * max|ref| (errors average down over the pixel reduction)."""
 import pytest
@@ -15,7 +15,7 @@ SHAPES = [  # B, Cin, H, W, Cout, k, stride, pad
     (2, 16, 15, 15, 24, 3, 1, 1),
     (2, 16, 14, 14, 32, 1, 2, 0),
     (1, 3, 33, 33, 16, 7, 2, 3),
-    (3, 40, 9, 9, 200, 3, 1, 1),        # Cout > 128: two n-tiles of TMEM lanes
+    (3, 40, 9, 9, 200, 3, 1, 1),        # Cout > 128: two 128-channel tiles
     (1, 1, 5, 5, 1, 5, 1, 0),
     (3, 64, 12, 12, 64, 3, 1, 1),       # TMA-staged operands: one 64-channel chunk per tap, padding taps
     (2, 128, 9, 9, 96, 3, 1, 1),        # two chunks per tap, 18 atoms = 4.5 column tiles

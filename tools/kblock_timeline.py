@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Per-k-block hand-off timeline of the tiled tcgen05 kernel (NN_UMMA_KDEBUG=1): for every k-block of every CTA, when
-producer thread 0 woke from the empty barrier / arrived on the full barrier, and when the MMA thread woke / committed.
+"""Per-k-block hand-off timeline of the tiled wgmma kernel (NN_UMMA_KDEBUG=1): for every k-block of every CTA, when
+producer thread 0 woke from the empty barrier / arrived on the full barrier, and when the first MMA warpgroup woke / released the stage.
 The stamps are compiled in only with -DNN_KDEBUG:  NN_EXTRA_NVCC=-DNN_KDEBUG python __graft_entry__.py --force"""
 import ctypes as C
 import os
@@ -31,12 +31,12 @@ for name, fn, ctas, nkb in (("conv2 dgrad", lambda: ops.conv_dgrad(gy, wq, (B, 6
     print("%s: %d CTAs with stamps" % (name, t.shape[0]))
     build = (t[:, :, 1] - t[:, :, 0]) * us
     mma = (t[:, :, 3] - t[:, :, 2]) * us
-    p2m = (t[:, :, 2] - t[:, :, 1]) * us                  # producer arrived -> MMA thread woke (same k-block)
+    p2m = (t[:, :, 2] - t[:, :, 1]) * us                  # producer arrived -> MMA warpgroup woke (same k-block)
     per_p = np.diff(t[:, :, 0], axis=1) * us
     per_m = np.diff(t[:, :, 2], axis=1) * us
     m2p = (t[:, 2:, 0] - t[:, :-2, 3]) * us              # MMA committed k-block kb -> producer woke for kb + 2 (2 stages)
-    for lab, a in (("producer: wake -> arrive (issue 8 chunk copies)", build), ("producer arrive -> MMA thread awake", p2m),
-                   ("MMA thread: awake -> committed", mma), ("MMA commit(kb) -> producer awake for kb+stages", m2p),
+    for lab, a in (("producer: wake -> arrive (issue 8 chunk copies)", build), ("producer arrive -> MMA warpgroup awake", p2m),
+                   ("MMA warpgroup: awake -> stage released", mma), ("stage release(kb) -> producer awake for kb+stages", m2p),
                    ("k-block period (producer)", per_p), ("k-block period (MMA)", per_m)):
         print("   %-52s mean %6.3f us  p10 %6.3f  p50 %6.3f  p90 %6.3f" % (lab, a.mean(), np.percentile(a, 10), np.percentile(a, 50), np.percentile(a, 90)))
     print("   CTA main-loop span: mean %.1f us" % ((t[:, -1, 3] - t[:, 0, 0]) * us).mean())

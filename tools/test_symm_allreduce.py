@@ -26,7 +26,7 @@ class Toy(torch.nn.Module):
 
 
 def log(rank, msg):
-    with open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out", "symm_rank%d.log" % rank), "a") as f:
+    with open("symm_rank%d.log" % rank, "a") as f:          # per-rank progress log in the working directory
         f.write(msg + "\n")
 
 
