@@ -10,8 +10,11 @@
 //   zero-filled by the TMA unit: no thread computes an address.
 // * B operand: pre-swizzled weight image [n-tile][tap][group][half][chunk rows]; per stage and chunk two tiled
 //   tensor-map copies (the two row halves) land the chunk's n_mma rows contiguously.
-// * Persistent: a CTA walks (128-pixel tile, n-tile) items.  Two MMA warpgroups (64 pixels each) accumulate the main
-//   and sigma^2 columns in registers and run the epilogue (scale, Philox / Box-Muller current noise -> NCHW stores)
+// * CTA pairs: clusters of two CTAs walk adjacent 128-pixel tiles of one n-tile in lockstep; each multicasts one of the
+//   two weight row halves to both, so the weights (65 % of the operand bytes of conv2's forward) cross L2 once per pair.
+// * Persistent: a pair walks (two 128-pixel tiles, n-tile) items.  Two MMA warpgroups (64 pixels each) accumulate the
+//   main and sigma^2 columns in registers with ONE wgmma per k16 step over the full width (m64n240k16 for conv2), keep
+//   one ring stage's wgmmas in flight, and run the epilogue (scale, Philox / Box-Muller current noise -> NCHW stores)
 //   straight from the wgmma fragments, while the producers already fill the ring with the next item's operands.
 // * Warp roles: warps 0-7 the two MMA / epilogue warpgroups, warps 8 .. 8 + P - 1 producers (one elected thread each; a
 //   thread owns whole stages round-robin, since a tensor-map copy keeps its issuing thread busy for hundreds of cycles).
@@ -30,8 +33,8 @@ struct TmaConvP {
     CUtensorMap mapb64, mapb_tail;       // weight image as rows of 128 B / of the tail width: boxes of n_half rows
     int M, OH, OW, Cout, stride, pad, KW, taps;
     int n_c64, tail_w, nc, gpt, n_groups;
-    int n_t, n_mma, n_half, n_tiles;
-    int items, stages, a_stage, b_stage, n_prod, tap_bytes;
+    int n_mma, n_half, n_tiles;
+    int stages, a_stage, b_stage, n_prod, tap_bytes;
     float y_scale, s_scale;
     float *y, *y_noisy;
     float current;
@@ -41,11 +44,29 @@ struct TmaConvP {
     int* err_flag;
 };
 
-// EPI 1: noisy (main + sigma accumulators, Philox z), EPI 2: plain, EPI 3: noisy with injected z (parity tests)
-template <int EPI>
+// The wgmmas of one ring stage of k_conv_tma: KA k16 steps of the stage's first channel chunk, KB of its second (0: none),
+// committed as one group; returns when the previous stage's group has completed.  scale_d of the first one: 0 starts the
+// accumulators of an item.
+template <int N, int KA, int KB>
+__device__ __forceinline__ void conv_stage_mma(float* acc, uint64_t ad_a, uint64_t bd_a, uint64_t ad_b, uint64_t bd_b, int acc0) {
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < KA; ++k) wgmma_c<N, 0, 0>(acc, ad_a + 2 * k, bd_a + 2 * k, k == 0 ? acc0 : 1);
+#pragma unroll
+    for (int k = 0; k < KB; ++k) wgmma_c<N, 0, 0>(acc, ad_b + 2 * k, bd_b + 2 * k, 1);
+    wg_commit();
+    wg_wait_1();            // this stage's wgmmas stay in flight; the previous stage's have completed
+}
+
+// EPI 1: noisy (main + sigma accumulators, Philox z), EPI 2: plain, EPI 3: noisy with injected z (parity tests).
+// NT = main accumulator columns of an n-tile (the plan's n_t); the MMA width is NT, or 2 NT with the sigma^2 columns.
+// Launched as clusters of two CTAs (rank r = 0 / 1) that walk adjacent m-tiles (2 mp + r) of the same n-tile in lockstep:
+// each producer copies its own A and multicasts weight row half r to both CTAs, so a weight stage crosses L2 once per pair.
+template <int EPI, int NT>
 __global__ void __launch_bounds__((8 + 2) * 32, 1)
 k_conv_tma(const __grid_constant__ TmaConvP p) {
-    constexpr int MCH = EPI == 2 ? 4 : 2;        // 64-column register chunks of the main / sigma accumulators
+    constexpr bool noise = EPI != 2;
+    constexpr int N = noise ? 2 * NT : NT;       // one wgmma per k16 step: [main | sigma^2] columns (fragment offset NT / 2)
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const int S = p.stages;
@@ -56,11 +77,14 @@ k_conv_tma(const __grid_constant__ TmaConvP p) {
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);          // warp-uniform for the compiler: role branches are convergent
     const int P = p.n_prod;
+    const uint32_t rank = cluster_ctarank(), peer = rank ^ 1u;
+    const int n_mt = (p.M + 127) >> 7, pairs = ((n_mt + 1) >> 1) * p.n_tiles;
+    const int cl0 = blockIdx.x >> 1, n_cl = gridDim.x >> 1;
 
     if (tid == 0) {
         for (int s = 0; s < S; ++s) {
-            mbar_init(full_bar + 8 * s, 1);          // the producer's arrive.expect_tx
-            mbar_init(empty_bar + 8 * s, 2);         // both MMA warpgroups have read the stage
+            mbar_init(full_bar + 8 * s, 1);          // the producer's arrive.expect_tx (A + both weight halves)
+            mbar_init(empty_bar + 8 * s, 4);         // both MMA warpgroups of both CTAs have read the stage
         }
         fence_mbar_init();
         tma_prefetch_desc(&p.map64);
@@ -68,7 +92,7 @@ k_conv_tma(const __grid_constant__ TmaConvP p) {
         tma_prefetch_desc(&p.mapb64);
         tma_prefetch_desc(&p.mapb_tail);
     }
-    __syncthreads();
+    cluster_sync();                                  // the peer's barriers are initialised before any copy or arrival reaches them
     const int ohw = p.OH * p.OW;
 
     if (warp >= 8 && warp < 8 + P) {
@@ -78,8 +102,10 @@ k_conv_tma(const __grid_constant__ TmaConvP p) {
         uint32_t eph = 1u;                                   // parity to wait for on the stage's empty barrier
         // (no function call inside the role loops: uniform registers do not survive calls -- the loops break out instead)
         int fail = 0;
-        for (int it = blockIdx.x; it < p.items && !fail; it += gridDim.x) {
-            const int mt = it / p.n_tiles, nt = it - mt * p.n_tiles;
+        for (int pi = cl0; pi < pairs && !fail; pi += n_cl) {
+            const int mp = pi / p.n_tiles, nt = pi - mp * p.n_tiles;
+            // the odd last m-tile: rank 1 reloads its partner's A (no stores follow) because the partner needs its weight half
+            const int mt = min(2 * mp + (int)rank, n_mt - 1);
             const int m0 = mt * 128;
             const int b0 = m0 / ohw, r0 = m0 - b0 * ohw, oh0 = r0 / p.OW, ow0 = r0 - oh0 * p.OW;
             const int iw0 = ow0 * p.stride - p.pad, ih0 = oh0 * p.stride - p.pad;
@@ -100,18 +126,18 @@ k_conv_tma(const __grid_constant__ TmaConvP p) {
                         if (wb) tma_im2col_4d(a_dst + 256u * (uint32_t)wa, cb < p.n_c64 ? &p.map64 : &p.map_tail, bar, 64 * cb, iw0, ih0, b0,
                                               (uint16_t)kw, (uint16_t)kh);
                         const int tap = kh * p.KW + kw;
-                        // chunk a of the group: rows [half 0 | half 1] at b_dst; chunk b after all n_mma rows of chunk a
-                        for (int h = 0; h < 2; ++h) {
-                            const long long boff = wt + (long long)tap * p.tap_bytes + (long long)gi * (p.n_half * 512) + (long long)h * half_bytes;
-                            const uint32_t da = b_dst + (uint32_t)(h * p.n_half * 2 * wa);
-                            if (wa == 64) tma_tile_2d(da, &p.mapb64, bar, 0, (int)(boff >> 7));
-                            else tma_tile_2d(da, &p.mapb_tail, bar, 0, (int)(boff / (2 * wa)));
-                            if (wb) {
-                                const long long boff2 = boff + (long long)p.n_half * 2 * wa;
-                                const uint32_t db = b_dst + (uint32_t)(p.n_mma * 2 * wa + h * p.n_half * 2 * wb);
-                                if (wb == 64) tma_tile_2d(db, &p.mapb64, bar, 0, (int)(boff2 >> 7));
-                                else tma_tile_2d(db, &p.mapb_tail, bar, 0, (int)(boff2 / (2 * wb)));
-                            }
+                        // chunk a of the group: rows [half 0 | half 1] at b_dst; chunk b after all n_mma rows of chunk a.
+                        // This CTA's half (h = rank) goes to both CTAs of the pair.
+                        const int h = (int)rank;
+                        const long long boff = wt + (long long)tap * p.tap_bytes + (long long)gi * (p.n_half * 512) + (long long)h * half_bytes;
+                        const uint32_t da = b_dst + (uint32_t)(h * p.n_half * 2 * wa);
+                        if (wa == 64) tma_tile_2d_mc(da, &p.mapb64, bar, 0, (int)(boff >> 7), 0x3);
+                        else tma_tile_2d_mc(da, &p.mapb_tail, bar, 0, (int)(boff / (2 * wa)), 0x3);
+                        if (wb) {
+                            const long long boff2 = boff + (long long)p.n_half * 2 * wa;
+                            const uint32_t db = b_dst + (uint32_t)(p.n_mma * 2 * wa + h * p.n_half * 2 * wb);
+                            if (wb == 64) tma_tile_2d_mc(db, &p.mapb64, bar, 0, (int)(boff2 >> 7), 0x3);
+                            else tma_tile_2d_mc(db, &p.mapb_tail, bar, 0, (int)(boff2 / (2 * wb)), 0x3);
                         }
                     }
                     __syncwarp();
@@ -126,55 +152,67 @@ k_conv_tma(const __grid_constant__ TmaConvP p) {
     } else if (warp < 8) {
         // ---------------------------------------------------------------- MMA warpgroups + epilogue
         const int wg = warp >> 2, wt = tid & 127;
-        constexpr bool noise = EPI != 2;
         float coef = 0.f;
         NnRng rs = {0, 0, 0, 0};
         if (noise) { coef = nn_noise_coef(*p.scale_dev, p.current); rs = nn_rng_load(p.rng); }
         const int ngrp = (p.Cout + 3) >> 2;
         const float y_scale = p.y_scale, s_scale = p.s_scale;
         const int kt = p.tail_w >> 4;
+        const bool releaser = (warp & 3) == 0;
         int s = 0, fail = 0;
         uint32_t fph = 0u;                                   // parity to wait for on the stage's full barrier
-        for (int it = blockIdx.x; it < p.items && !fail; it += gridDim.x) {
-            const int mt = it / p.n_tiles, nt = it - mt * p.n_tiles;
-            float accm[MCH][32], accs[2][32];
-            int gi = 0;
+        for (int pi = cl0; pi < pairs && !fail; pi += n_cl) {
+            const int mp = pi / p.n_tiles, nt = pi - mp * p.n_tiles;
+            const int mt = 2 * mp + (int)rank;
+            float acc[N / 2];
+            int gi = 0, prev = 0;
             for (int g = 0; g < p.n_groups; ++g) {
                 if (!mbar_wait(full_bar + 8 * s, fph)) { fail = 403; break; }
                 const int ca = 2 * gi, cb = 2 * gi + 1;
                 const bool has_b = cb < p.nc;
+                const int wa = ca < p.n_c64 ? 64 : p.tail_w, wb = has_b ? (cb < p.n_c64 ? 64 : p.tail_w) : 0;
                 const uint32_t a_s = base + (uint32_t)s * stage_bytes, b_s = a_s + (uint32_t)p.a_stage;
-                wg_fence();
-#pragma unroll 1
-                for (int ch = 0; ch < (has_b ? 2 : 1); ++ch) {
-                    const int w = (ch == 0 ? ca : cb) < p.n_c64 ? 64 : p.tail_w;      // channels of this chunk (row = 2 w bytes)
-                    const uint32_t a_c = a_s + (ch == 0 ? 0u : 256u * (uint32_t)(ca < p.n_c64 ? 64 : p.tail_w));
-                    const uint32_t b_c = b_s + (ch == 0 ? 0u : (uint32_t)(p.n_mma * 2 * (ca < p.n_c64 ? 64 : p.tail_w)));
-                    const uint64_t ad = gmma_desc_kmajor(a_c + (uint32_t)(wg * 64 * 2 * w), 2u * (uint32_t)w);
-                    const uint64_t bm = gmma_desc_kmajor(b_c, 2u * (uint32_t)w);
-                    const uint64_t bsg = gmma_desc_kmajor(b_c + (uint32_t)(p.n_t * 2 * w), 2u * (uint32_t)w);    // sigma rows follow the main rows
-                    const uint32_t step = 8u * (uint32_t)w;               // 64 rows of B in descriptor units
-                    const int ks = w == 64 ? 4 : kt;
-#pragma unroll 1
-                    for (int k = 0; k < ks; ++k) {
-                        const int acc_on = (g != 0 || ch != 0 || k != 0) ? 1 : 0;
-                        wg_mma<MCH, 0, 0>(accm, ad + 2 * k, bm + 2 * k, step, p.n_t, acc_on);
-                        if (noise) wg_mma<2, 0, 0>(accs, ad + 2 * k, bsg + 2 * k, step, p.n_t, acc_on);
-                    }
+                // chunk a: A at a_s, B at b_s (main rows, then the sigma^2 rows); chunk b: A after chunk a's 128 rows, B after
+                // its n_mma rows.  K-major tiles with rows of 2 w bytes.
+                const uint64_t ad_a = gmma_desc_kmajor(a_s + (uint32_t)(wg * 64 * 2 * wa), 2u * (uint32_t)wa);
+                const uint64_t bd_a = gmma_desc_kmajor(b_s, 2u * (uint32_t)wa);
+                const uint32_t a_b = a_s + 256u * (uint32_t)wa, b_b = b_s + (uint32_t)(p.n_mma * 2 * wa);
+                const uint64_t ad_b = has_b ? gmma_desc_kmajor(a_b + (uint32_t)(wg * 64 * 2 * wb), 2u * (uint32_t)wb) : 0;
+                const uint64_t bd_b = has_b ? gmma_desc_kmajor(b_b, 2u * (uint32_t)wb) : 0;
+                const int ka = wa == 64 ? 4 : kt, kb = wb == 64 ? 4 : (wb ? kt : 0);
+                const int acc0 = g != 0 ? 1 : 0;
+                // one straight-line sequence per stage shape (k16 steps of chunks a, b), fence to wait: a branch or a loop back
+                // edge between two wgmmas, or between them and the wait, makes ptxas insert a warpgroup.arrive there
+                switch (8 * ka + kb) {
+                    case 8 * 4 + 4: conv_stage_mma<N, 4, 4>(acc, ad_a, bd_a, ad_b, bd_b, acc0); break;
+                    case 8 * 4 + 2: conv_stage_mma<N, 4, 2>(acc, ad_a, bd_a, ad_b, bd_b, acc0); break;
+                    case 8 * 4 + 1: conv_stage_mma<N, 4, 1>(acc, ad_a, bd_a, ad_b, bd_b, acc0); break;
+                    case 8 * 4: conv_stage_mma<N, 4, 0>(acc, ad_a, bd_a, ad_b, bd_b, acc0); break;
+                    case 8 * 2: conv_stage_mma<N, 2, 0>(acc, ad_a, bd_a, ad_b, bd_b, acc0); break;
+                    default: conv_stage_mma<N, 1, 0>(acc, ad_a, bd_a, ad_b, bd_b, acc0); break;      // 8 * 1: a 16-channel tail alone
                 }
-                wg_commit();
-                wg_wait_all();
-                wg_fence_acc(accm);
-                if (noise) wg_fence_acc(accs);
+                // the previous stage's operands may be refilled
+                if (g != 0 && releaser && elect_one_sync()) {
+                    mbar_arrive(empty_bar + 8 * prev);
+                    mbar_arrive_cluster(cluster_map(empty_bar + 8 * prev, peer));
+                }
                 __syncwarp();
-                if ((warp & 3) == 0 && elect_one_sync()) mbar_arrive(empty_bar + 8 * s);      // the stage may be refilled
-                __syncwarp();
+                prev = s;
                 if (++gi == p.gpt) gi = 0;
                 if (++s == S) { s = 0; fph ^= 1u; }
             }
             if (fail) break;
-            // ---- epilogue from the fragments: rows r0, r0 + 8; columns 8 i + 2 (l % 4) + {0, 1} of each chunk.  The two
-            // lanes l, l ^ 1 share the 4-channel Philox groups of both rows: each draws one and hands over half of it.
+            wg_wait_all();
+            wg_fence_regs<N / 2>(acc);
+            if (releaser && elect_one_sync()) {
+                mbar_arrive(empty_bar + 8 * prev);
+                mbar_arrive_cluster(cluster_map(empty_bar + 8 * prev, peer));
+            }
+            __syncwarp();
+            if (mt >= n_mt) continue;                        // rank 1's copy of the odd last m-tile: nothing to store
+            // ---- epilogue from the fragments: rows r0, r0 + 8; columns 8 i + 2 (l % 4) + {0, 1} (registers 4 i + 2 h + j;
+            // the sigma^2 partner of a main column NT / 2 registers later).  The two lanes l, l ^ 1 share the 4-channel
+            // Philox groups of both rows: each draws one and hands over half of it.
             const int r_top = 64 * wg + 16 * (wt >> 5) + (lane >> 2);
             const int m_a = mt * 128 + r_top, m_b = m_a + 8;
             const bool odd = (lane & 1) != 0;
@@ -189,44 +227,41 @@ k_conv_tma(const __grid_constant__ TmaConvP p) {
                 orow[h] = (size_t)b * p.Cout * ohw + pix;
             }
             float* const out = EPI != 2 ? p.y_noisy : p.y;
-            const int n_base = nt * p.n_t;
+            const int n_base = nt * NT;
 #pragma unroll
-            for (int c = 0; c < MCH; ++c)
+            for (int i = 0; i < NT / 8; ++i) {
+                const int n = n_base + 8 * i + 2 * (lane & 3);        // column of register 4 i (+1: next column)
+                float z[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+                if (EPI == 1) {
+                    float zz[4];
+                    nn_normal4(rs, (uint64_t)m_own * ngrp + (uint64_t)(n >> 2), zz);
+                    // even lane keeps z[0..1] of row a, gets z[0..1] of row b; odd lane keeps z[2..3] of row b, gets those of row a
+                    const float o0 = __shfl_xor_sync(0xffffffffu, odd ? zz[0] : zz[2], 1);
+                    const float o1 = __shfl_xor_sync(0xffffffffu, odd ? zz[1] : zz[3], 1);
+                    if (odd) { z[0][0] = o0; z[0][1] = o1; z[1][0] = zz[2]; z[1][1] = zz[3]; }
+                    else { z[0][0] = zz[0]; z[0][1] = zz[1]; z[1][0] = o0; z[1][1] = o1; }
+                }
 #pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const int nl = 64 * c + 8 * i + 2 * (lane & 3);        // local column of register 4 i (+1: next column)
-                    if (64 * c + 8 * i >= p.n_t) continue;                 // warp-uniform
-                    const int n = n_base + nl;
-                    float z[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
-                    if (EPI == 1) {
-                        float zz[4];
-                        nn_normal4(rs, (uint64_t)m_own * ngrp + (uint64_t)(n >> 2), zz);
-                        // even lane keeps z[0..1] of row a, gets z[0..1] of row b; odd lane keeps z[2..3] of row b, gets those of row a
-                        const float o0 = __shfl_xor_sync(0xffffffffu, odd ? zz[0] : zz[2], 1);
-                        const float o1 = __shfl_xor_sync(0xffffffffu, odd ? zz[1] : zz[3], 1);
-                        if (odd) { z[0][0] = o0; z[0][1] = o1; z[1][0] = zz[2]; z[1][1] = zz[3]; }
-                        else { z[0][0] = zz[0]; z[0][1] = zz[1]; z[1][0] = o0; z[1][1] = o1; }
-                    }
+                for (int h = 0; h < 2; ++h) {
+                    if (!ok[h]) continue;
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        if (!ok[h]) continue;
-#pragma unroll
-                        for (int j = 0; j < 2; ++j) {
-                            if (nl + j >= p.n_t || n + j >= p.Cout) continue;
-                            const size_t o = orow[h] + (size_t)(n + j) * ohw;
-                            const float yv = accm[c][4 * i + 2 * h + j] * y_scale;
-                            if (EPI == 2) {
-                                out[o] = yv;
-                            } else {
-                                const float zv = EPI == 3 ? __ldg(p.z_inject + o) : z[h][j];
-                                out[o] = __fadd_rn(yv, __fmul_rn(zv, nn_sigma(coef, accs[c & 1][4 * i + 2 * h + j] * s_scale)));      // (MCH == 2)
-                            }
+                    for (int j = 0; j < 2; ++j) {
+                        if (n + j >= p.Cout) continue;
+                        const size_t o = orow[h] + (size_t)(n + j) * ohw;
+                        const float yv = acc[4 * i + 2 * h + j] * y_scale;
+                        if (EPI == 2) {
+                            out[o] = yv;
+                        } else {
+                            const float zv = EPI == 3 ? __ldg(p.z_inject + o) : z[h][j];
+                            out[o] = __fadd_rn(yv, __fmul_rn(zv, nn_sigma(coef, acc[N / 4 + 4 * i + 2 * h + j] * s_scale)));
                         }
                     }
                 }
+            }
         }
         if (fail) nn_pipeline_abort(p.err_flag, fail);
     }
+    cluster_sync();                                  // neither CTA exits while its peer can still write to it or arrive on it
 }
 
 typedef CUresult (*EncodeIm2colFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const int*,
@@ -293,6 +328,42 @@ int encode_weight_map(CUtensorMap* map, const void* wp, size_t wp_bytes, int row
 }
 
 int g_tma_enable = 1;
+
+typedef void (*TmaConvKernel)(const TmaConvP);
+
+// k_conv_tma<EPI, NT> for NT = nt: every n-tile width a plan can produce (multiples of 8 up to NMAX)
+template <int EPI, int NT, int NMAX>
+TmaConvKernel tma_conv_kernel(int nt) {
+    if (nt == NT) return k_conv_tma<EPI, NT>;
+    if constexpr (NT + 8 <= NMAX) return tma_conv_kernel<EPI, NT + 8, NMAX>(nt);
+    else return nullptr;
+}
+
+// once per (device, kernel): the shared-memory opt-in; once per (device, shared-memory size): the number of co-resident
+// clusters (an occupancy query of one kernel stands for all: same block size, one CTA per SM whatever the width)
+int tma_conv_prepare(TmaConvKernel kern, int device, const cudaLaunchConfig_t& cfg, int* n_cl) {
+    struct Seen { int device; TmaConvKernel kern; };
+    struct Occ { int device; size_t smem; int clusters; };
+    static Seen seen[256];
+    static Occ occ[32];
+    static int n_seen = 0, n_occ = 0;
+    bool done = false;
+    for (int i = 0; i < n_seen && !done; ++i) done = seen[i].device == device && seen[i].kern == kern;
+    if (!done) {
+        NN_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        if (n_seen < 256) seen[n_seen++] = {device, kern};
+    }
+    for (int i = 0; i < n_occ; ++i)
+        if (occ[i].device == device && occ[i].smem == cfg.dynamicSmemBytes) { *n_cl = occ[i].clusters; return 0; }
+    cudaLaunchConfig_t q = cfg;
+    q.gridDim = dim3(2 * nn_num_sms(device));
+    int n = 0;
+    NN_CUDA_OK(cudaOccupancyMaxActiveClusters(&n, kern, &q));
+    if (n < 1) return nn_fail("nn_conv_tma: no cluster of two CTAs fits on the device%s", "");
+    if (n_occ < 32) occ[n_occ++] = {device, cfg.dynamicSmemBytes, n};
+    *n_cl = n;
+    return 0;
+}
 
 }  // namespace
 
@@ -367,22 +438,35 @@ int nn_tma_conv_launch(const TmaConvCall& c, int device, cudaStream_t st) {
     if (pl.tail_w == 0) p.mapb_tail = p.mapb64;
     p.M = c.B * c.OH * c.OW; p.OH = c.OH; p.OW = c.OW; p.Cout = c.Cout; p.stride = c.stride; p.pad = c.pad; p.KW = c.KW; p.taps = pl.taps;
     p.n_c64 = pl.n_c64; p.tail_w = pl.tail_w; p.nc = pl.nc; p.gpt = pl.gpt; p.n_groups = pl.n_groups;
-    p.n_t = pl.n_t; p.n_mma = pl.n_mma; p.n_half = pl.n_half; p.n_tiles = pl.n_tiles;
-    p.items = ((p.M + 127) / 128) * pl.n_tiles;
+    p.n_mma = pl.n_mma; p.n_half = pl.n_half; p.n_tiles = pl.n_tiles;
     p.stages = pl.stages; p.a_stage = pl.a_stage; p.b_stage = pl.b_stage; p.n_prod = pl.n_prod; p.tap_bytes = pl.tap_bytes;
     p.y_scale = c.y_scale; p.s_scale = c.s_scale; p.y = c.y; p.y_noisy = c.y_noisy;
     p.current = c.current; p.scale_dev = c.scale_dev; p.z_inject = c.z_inject; p.rng = c.rng; p.err_flag = c.err_flag;
-    int grid = nn_num_sms(device);          // persistent: one CTA per SM
-    if (grid > p.items) grid = p.items;
-    NN_ONCE_PER_DEVICE({
-        NN_CUDA_OK(cudaFuncSetAttribute(k_conv_tma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        NN_CUDA_OK(cudaFuncSetAttribute(k_conv_tma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        NN_CUDA_OK(cudaFuncSetAttribute(k_conv_tma<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    });
+    const bool noise = c.noise_mode != NN_NOISE_NONE;
+    const int epi = noise ? (c.z_inject ? 3 : 1) : 2;
+    const TmaConvKernel kern = epi == 3 ? tma_conv_kernel<3, 8, 128>(pl.n_t) : epi == 1 ? tma_conv_kernel<1, 8, 128>(pl.n_t)
+                                                                             : tma_conv_kernel<2, 8, 256>(pl.n_t);
+    if (!kern) return nn_fail("nn_conv_tma: no kernel for an n-tile of%s %lld columns", "", (long long)pl.n_t);
+    // persistent clusters of two CTAs (one CTA per SM): as many as fit at once, at most one per pair of m-tiles and n-tile
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.blockDim = dim3(pl.threads);
+    cfg.dynamicSmemBytes = pl.smem_bytes;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int n_cl = 0;
+    if (int e = tma_conv_prepare(kern, device, cfg, &n_cl)) return e;
+    const int pairs = ((p.M + 255) / 256) * pl.n_tiles;
+    if (n_cl > pairs) n_cl = pairs;
+    cfg.gridDim = dim3(2 * n_cl);
     if (c.ev0) cudaEventRecord((cudaEvent_t)c.ev0, st);          // measurement hook: brackets the kernel, not the host-side descriptor encoding
-    if (c.noise_mode != NN_NOISE_NONE && c.z_inject) k_conv_tma<3><<<grid, pl.threads, pl.smem_bytes, st>>>(p);
-    else if (c.noise_mode != NN_NOISE_NONE) k_conv_tma<1><<<grid, pl.threads, pl.smem_bytes, st>>>(p);
-    else k_conv_tma<2><<<grid, pl.threads, pl.smem_bytes, st>>>(p);
+    NN_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
     if (c.ev1) cudaEventRecord((cudaEvent_t)c.ev1, st);
     NN_LAUNCH_OK();
     return 0;
@@ -432,7 +516,41 @@ constexpr int WT_STAGE = 16384 + 32768;        // A: 2 atoms, B: 4 atoms of 8 KB
 constexpr int WT_PROD = 4;                     // producer warps (warps 0-7 MMA warpgroups, 8-11 producers)
 constexpr int WT_THREADS = (8 + WT_PROD) * 32;
 
-template <bool TAIL>
+// the MMA warpgroups' k-block loop at a compile-time width N (one wgmma per k16 step); returns a watchdog code or 0
+template <int N, bool TAIL>
+__device__ __forceinline__ int wgrad_mma_loop(float* acc, int nkb, uint32_t base, uint32_t full_bar, uint32_t empty_bar, int S, int wg,
+                                              bool releaser) {
+    // A: SWIZZLE_128B MN-major atoms (LBO = atom stride 8192 B, 16 pixels = 2048 B); B: main -- the same; remainder slab --
+    // LBO = 8-pixel groups 128 B apart, SBO = the taps' slabs 1 KB apart, 16 pixels = 256 B
+    const uint64_t da = gmma_desc(0u, 8192u >> 4, 1024u >> 4, 1u);
+    const uint64_t db = TAIL ? gmma_desc(0u, 8u, 64u, 0u) : da;
+    constexpr uint32_t k_step_b = TAIL ? 16u : 128u;
+    int s = 0, prev = 0;
+    uint32_t ph = 0u;
+    for (int i = 0; i < nkb; ++i) {
+        if (!mbar_wait(full_bar + 8 * s, ph)) return 502;
+        const uint32_t a_s = (base + (uint32_t)s * WT_STAGE + (uint32_t)wg * 8192u) >> 4, b_s = (base + (uint32_t)s * WT_STAGE + 16384u) >> 4;
+        const uint64_t ad = da | (uint64_t)(a_s & 0x3FFFu), bd = db | (uint64_t)(b_s & 0x3FFFu);
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_c<N, 1, 1>(acc, ad + 128 * k, bd + k_step_b * k, (i | k) != 0 ? 1 : 0);
+        wg_commit();
+        wg_wait_1();                     // this k-block's wgmmas stay in flight; the previous block's stage is released
+        if (i != 0 && releaser && elect_one_sync()) mbar_arrive(empty_bar + 8 * prev);
+        __syncwarp();
+        prev = s;
+        if (++s == S) { s = 0; ph ^= 1u; }
+    }
+    wg_wait_all();
+    wg_fence_regs<N / 2>(acc);
+    if (nkb > 0 && releaser && elect_one_sync()) mbar_arrive(empty_bar + 8 * prev);
+    __syncwarp();
+    return 0;
+}
+
+// TW: the MMA width of the remainder launch (TAIL; 16 * ceil(taps / 2) columns), 0 for the main launch, whose column
+// tiles have 1 .. 4 atoms of 64 columns (the last tile of a layer is narrower): one compile-time width per case
+template <bool TAIL, int TW>
 __global__ void __launch_bounds__(WT_THREADS, 1)
 k_wgrad_tma(const __grid_constant__ WgTmaP p) {
     extern __shared__ uint8_t smem_raw[];
@@ -490,30 +608,14 @@ k_wgrad_tma(const __grid_constant__ WgTmaP p) {
         }
     } else {
         // ---- MMA warpgroups: MN-major A and B; warpgroup g owns output channels 64 g .. 64 g + 63 (the second atom of A, + 8 KB).
-        // B: main -- SWIZZLE_128B atoms (LBO = atom stride 8192 B, 16 pixels = 2048 B); remainder slab -- LBO = 8-pixel groups
-        // 128 B apart, SBO = the taps' slabs 1 KB apart, 16 pixels = 256 B
         const int wg = warp >> 2;
-        const uint64_t da = gmma_desc(0u, 8192u >> 4, 1024u >> 4, 1u);
-        const uint64_t db = TAIL ? gmma_desc(0u, 8u, 64u, 0u) : da;
-        const uint32_t b_step = 512u, k_step_b = TAIL ? 16u : 128u;
-        float acc[4][32];
-        int s = 0;
-        uint32_t ph = 0u;
-        for (int i = 0; i < nkb; ++i) {
-            if (!mbar_wait(full_bar + 8 * s, ph)) { fail = 502; break; }
-            const uint32_t a_s = (base + (uint32_t)s * WT_STAGE + (uint32_t)wg * 8192u) >> 4, b_s = (base + (uint32_t)s * WT_STAGE + 16384u) >> 4;
-            const uint64_t ad = da | (uint64_t)(a_s & 0x3FFFu), bd = db | (uint64_t)(b_s & 0x3FFFu);
-            wg_fence();
-#pragma unroll
-            for (int k = 0; k < 4; ++k) wg_mma<4, 1, 1>(acc, ad + 128 * k, bd + k_step_b * k, b_step, n_cols, (i | k) != 0 ? 1 : 0);
-            wg_commit();
-            wg_wait_all();
-            wg_fence_acc(acc);
-            __syncwarp();
-            if ((warp & 3) == 0 && elect_one_sync()) mbar_arrive(empty_bar + 8 * s);
-            __syncwarp();
-            if (++s == S) { s = 0; ph ^= 1u; }
-        }
+        const bool releaser = (warp & 3) == 0;
+        float acc[128];
+        if constexpr (TAIL) fail = wgrad_mma_loop<TW, true>(acc, nkb, base, full_bar, empty_bar, S, wg, releaser);
+        else if (atoms == 4) fail = wgrad_mma_loop<256, TAIL>(acc, nkb, base, full_bar, empty_bar, S, wg, releaser);
+        else if (atoms == 3) fail = wgrad_mma_loop<192, TAIL>(acc, nkb, base, full_bar, empty_bar, S, wg, releaser);
+        else if (atoms == 2) fail = wgrad_mma_loop<128, TAIL>(acc, nkb, base, full_bar, empty_bar, S, wg, releaser);
+        else fail = wgrad_mma_loop<64, TAIL>(acc, nkb, base, full_bar, empty_bar, S, wg, releaser);
         if (!fail) {
             // ---- epilogue: rows = output channels, columns = (atom, channel) [or (tap, remainder channel)]
             const int wt = tid & 127;
@@ -530,7 +632,7 @@ k_wgrad_tma(const __grid_constant__ WgTmaP p) {
                     for (int j = 0; j < 8; ++j)
                         if (64 * c + 8 * j < n_cols)
                             *reinterpret_cast<float2*>(out + 64 * c + 8 * j) =
-                                nkb > 0 ? make_float2(acc[c][4 * j + 2 * h], acc[c][4 * j + 2 * h + 1]) : make_float2(0.f, 0.f);
+                                nkb > 0 ? make_float2(acc[32 * c + 4 * j + 2 * h], acc[32 * c + 4 * j + 2 * h + 1]) : make_float2(0.f, 0.f);
             }
         }
     }
@@ -618,14 +720,21 @@ int nn_tma_wgrad_launch(const TmaWgradCall& c, int device, cudaStream_t st) {
     p.OH = c.OH; p.OW = c.OW; p.stride = c.stride; p.pad = c.pad; p.KW = c.KW; p.n_c64 = w.n_c64; p.n_atoms = w.n_atoms;
     p.Mpix = c.B * c.OH * c.OW; p.Cout = c.Cout; p.num_kb = w.num_kb; p.kb_per_split = w.kb_per_split; p.stages = w.stages;
     p.cols_pad = w.cols_pad; p.partial = c.partial; p.err_flag = c.err_flag;
+    typedef void (*WgradKernel)(const WgTmaP);
+    // remainder launch: 8 columns per tap padded to 16 -- square filters of up to 5 x 5 (the plan's limit of 31 taps)
+    const int tw = w.tail_w ? (w.taps * 8 + 15) & ~15 : 0;
+    const WgradKernel tail = tw == 16 ? k_wgrad_tma<true, 16> : tw == 32 ? k_wgrad_tma<true, 32> : tw == 80 ? k_wgrad_tma<true, 80>
+                           : tw == 128 ? k_wgrad_tma<true, 128> : tw == 208 ? k_wgrad_tma<true, 208> : nullptr;
+    if (w.tail_w && !tail) return nn_fail("nn_conv_tma: no remainder weight-gradient kernel for%s %lld taps", "", (long long)w.taps);
     NN_ONCE_PER_DEVICE({
-        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_tma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        NN_CUDA_OK(cudaFuncSetAttribute(k_wgrad_tma<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+        for (WgradKernel k : {k_wgrad_tma<true, 16>, k_wgrad_tma<true, 32>, k_wgrad_tma<true, 80>, k_wgrad_tma<true, 128>, k_wgrad_tma<true, 208>})
+            NN_CUDA_OK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     });
-    k_wgrad_tma<false><<<dim3(w.tiles_k, w.m_tiles_n, w.splits), WT_THREADS, w.smem_bytes, st>>>(p);
+    k_wgrad_tma<false, 0><<<dim3(w.tiles_k, w.m_tiles_n, w.splits), WT_THREADS, w.smem_bytes, st>>>(p);
     NN_LAUNCH_OK();
     if (w.tail_w) {         // the 8-channel remainder columns of every tap: one column tile
-        k_wgrad_tma<true><<<dim3(1, w.m_tiles_n, w.splits), WT_THREADS, w.smem_bytes, st>>>(p);
+        tail<<<dim3(1, w.m_tiles_n, w.splits), WT_THREADS, w.smem_bytes, st>>>(p);
         NN_LAUNCH_OK();
     }
     return 0;

@@ -106,6 +106,31 @@ __device__ __forceinline__ void tma_prefetch_desc(const void* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
+// ------------------------------------------------------------------ thread-block clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// every thread of every CTA of the cluster; orders shared-memory writes (barrier inits) before the peers' accesses
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// the shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t cluster_map(uint32_t smem_addr, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
+}
+// tiled copy written to the same shared-memory offset of every CTA in `cta_mask`, completing on each one's barrier at `bar`
+__device__ __forceinline__ void tma_tile_2d_mc(uint32_t dst, const void* map, uint32_t bar, int c0, int c1, uint16_t cta_mask) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+                 ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask) : "memory");
+}
+
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
@@ -138,6 +163,8 @@ __device__ __forceinline__ uint64_t gmma_desc_none(uint32_t smem_addr, uint32_t 
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// all but the most recently committed group have completed: that group's operands are still being read
+__device__ __forceinline__ void wg_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 // keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
 template <int R>
 __device__ __forceinline__ void wg_fence_regs(float* d) {
@@ -145,84 +172,12 @@ __device__ __forceinline__ void wg_fence_regs(float* d) {
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n8(float* d, uint64_t a, uint64_t b, int scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0,%1,%2,%3}, %4, %5, p, 1, 1, %7, %8;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n16(float* d, uint64_t a, uint64_t b, int scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n24(float* d, uint64_t a, uint64_t b, int scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %14, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n24k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, %12, %13, p, 1, 1, %15, %16;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
-        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n32(float* d, uint64_t a, uint64_t b, int scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %19, %20;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n40(float* d, uint64_t a, uint64_t b, int scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %22, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n40k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19}, %20, %21, p, 1, 1, %23, %24;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
-        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n48(float* d, uint64_t a, uint64_t b, int scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n48k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1, %27, %28;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n56(float* d, uint64_t a, uint64_t b, int scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %30, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n56k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27}, %28, %29, p, 1, 1, %31, %32;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27])
-        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
-}
-template <int TA, int TB>
-__device__ __forceinline__ void wgmma_n64(float* d, uint64_t a, uint64_t b, int scale_d) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(a), "l"(b), "r"(scale_d), "n"(TA), "n"(TB));
-}
+}  // namespace
 
-// one wgmma of compile-time width N
-template <int N, int TA, int TB>
-__device__ __forceinline__ void wgmma_c(float* d, uint64_t a, uint64_t b, int scale_d) {
-    static_assert(N % 8 == 0 && N >= 8 && N <= 64, "wgmma_c: N = 8 .. 64");
-    if constexpr (N == 64) wgmma_n64<TA, TB>(d, a, b, scale_d);
-    else if constexpr (N == 56) wgmma_n56<TA, TB>(d, a, b, scale_d);
-    else if constexpr (N == 48) wgmma_n48<TA, TB>(d, a, b, scale_d);
-    else if constexpr (N == 40) wgmma_n40<TA, TB>(d, a, b, scale_d);
-    else if constexpr (N == 32) wgmma_n32<TA, TB>(d, a, b, scale_d);
-    else if constexpr (N == 24) wgmma_n24<TA, TB>(d, a, b, scale_d);
-    else if constexpr (N == 16) wgmma_n16<TA, TB>(d, a, b, scale_d);
-    else wgmma_n8<TA, TB>(d, a, b, scale_d);
-}
+#include "nn_wgmma_n.cuh"      // wgmma_n8 .. wgmma_n256 and wgmma_c<N>
+
+namespace {
+
 // one wgmma of runtime width n (a multiple of 8, <= 64) into the chunk registers d[32]
 template <int TA, int TB>
 __device__ __forceinline__ void wgmma_n(float* d, uint64_t a, uint64_t b, int n, int scale_d) {
