@@ -401,7 +401,7 @@ bool nn_tma_make_plan(int Cin_k, int KH, int KW, int stride, int pad, int n_out,
     if (pl.n_mma < 32) pl.n_mma = 32;
     if (pl.n_mma > 256) return false;
     pl.n_half = pl.n_mma / 2;
-    if (pl.n_t > (has_sigma ? 128 : 256)) return false;     // register accumulators of the MMA warpgroups
+    if (pl.n_t > (has_sigma ? 120 : 256)) return false;     // register accumulators of the MMA warpgroups
     int gw = 0;                                     // widest group of a tap (channels)
     for (int gi = 0; gi < pl.gpt; ++gi) {
         const int ca = 2 * gi, cb = 2 * gi + 1;
@@ -444,7 +444,7 @@ int nn_tma_conv_launch(const TmaConvCall& c, int device, cudaStream_t st) {
     p.current = c.current; p.scale_dev = c.scale_dev; p.z_inject = c.z_inject; p.rng = c.rng; p.err_flag = c.err_flag;
     const bool noise = c.noise_mode != NN_NOISE_NONE;
     const int epi = noise ? (c.z_inject ? 3 : 1) : 2;
-    const TmaConvKernel kern = epi == 3 ? tma_conv_kernel<3, 8, 128>(pl.n_t) : epi == 1 ? tma_conv_kernel<1, 8, 128>(pl.n_t)
+    const TmaConvKernel kern = epi == 3 ? tma_conv_kernel<3, 8, 120>(pl.n_t) : epi == 1 ? tma_conv_kernel<1, 8, 120>(pl.n_t)
                                                                              : tma_conv_kernel<2, 8, 256>(pl.n_t);
     if (!kern) return nn_fail("nn_conv_tma: no kernel for an n-tile of%s %lld columns", "", (long long)pl.n_t);
     // persistent clusters of two CTAs (one CTA per SM): as many as fit at once, at most one per pair of m-tiles and n-tile

@@ -21,7 +21,7 @@ SHAPES = [  # B, Cin, H, W, Cout, k, stride, pad
     (2, 128, 9, 9, 96, 3, 1, 1),        # two chunks per tap, 18 atoms = 4.5 column tiles
     (2, 64, 16, 16, 136, 3, 2, 1),      # stride 2, two n-tiles
     (2, 96, 10, 10, 24, 1, 2, 0),       # 1x1 stride 2, 64 + 32 channels (zero-filled second chunk)
-    (2, 72, 8, 8, 40, 3, 1, 1),         # 64 + 8 channels, 3 column tiles: remainder as a zero-filled chunk
+    (2, 72, 8, 8, 40, 3, 1, 1),         # 64 + 8 channels, 3 column tiles: the remainder accumulator (9 taps, 80 columns)
     (2, 72, 9, 9, 24, 5, 1, 2),         # 64 + 8 channels, 7 column tiles: the remainder accumulator (8 columns per tap), padding
     (3, 136, 8, 8, 16, 3, 2, 1),        # 128 + 8 channels, stride 2: remainder accumulator at channel 128
     (2, 136, 7, 7, 16, 1, 1, 0),        # 128 + 8 channels, 1x1
