@@ -492,14 +492,16 @@ k_splitk_epilogue(const SplitEpiP p) {
 // staged by ONE cp.async.bulk of (128 + (KH-1) W + KW-1) pixels = 4 KB instead of 64 KB of gathered im2col.
 // The whole weight image (taps x rows, 60 KB) stays resident in shared memory, so the CTA is persistent:
 //   warps 0 .. SH_EPI_WARPS - 1 : epilogue (scale, Philox/Box-Muller noise -> NCHW stores) from a shared-memory
-//              accumulator tile; the first 8 of them are also the two MMA warpgroups (64 tile rows each), one K = 16
-//              wgmma per PAIR of taps (LBO = pixel distance of the two taps), the N columns in 64-wide passes over the
-//              resident operands
-//   last warp : bulk-copy issuer (weights once, then the A ring, which runs ahead of the tiles)
-// The kernel is bound by the epilogue's instruction issue, not by data movement.
+//              accumulator tile; warps with (warp & 3) < 2 read its rows 0-63 (half 0), the others rows 64-127 (half 1)
+//   next 8 warps : two MMA warpgroups, one per 64-row half of the tile.  Each issues one K = 16 wgmma per PAIR of taps
+//              (LBO = pixel distance of the two taps) over the accumulator width, and stores its half into the tile as soon
+//              as that half's epilogue warps have released it -- so it runs up to one tile ahead of them.  The first warp of
+//              warpgroup 0 also issues the bulk copies (weights once, then the A ring, which runs ahead of the tiles).
+// 24 warps are 6 per SM sub-partition: a cap of 80 registers per thread, which both roles fit without spilling.
 constexpr int SH_MAX_PAIRS = 64;
 constexpr int SH_STAGES = 2;
 constexpr int SH_MAX_N = 256;                       // accumulator columns
+constexpr int SH_MAX_N1 = 80;                       // widest chain of one column pass (40 accumulators) under the 80-register cap
 constexpr int SH_POOL_IT = 5;                       // pooled launches: 4-channel groups per epilogue warp (<= 80 channels at 16 warps)
 
 struct ShiftP {
@@ -524,8 +526,15 @@ struct ShiftP {
     const float* scale_dev;
     nn_rng rng;
     int* err_flag;
-    long long* dbg;          // optional [cta][32 tiles][4] clock64 stamps: MMA ready / issued, accumulator seen / epilogue done
+    long long* dbg;          // optional [cta][32 tiles][SH_DBG] clock64 stamps (shift_dbg)
 };
+
+// debug stamps per tile (NN_KDEBUG builds, tools/shift_timeline.py): MMA warpgroup 0 A ready / half 0 stored, MMA warpgroup
+// 1 half 1 stored, epilogue warp 0 (half 0) accumulators seen / done, epilogue warp 2 (half 1) accumulators seen / done
+constexpr int SH_DBG = 8;
+__device__ __forceinline__ void shift_dbg(const ShiftP& p, int i, int k) {
+    if (p.dbg && i < 32) p.dbg[((size_t)blockIdx.x * 32 + i) * SH_DBG + k] = clock64();
+}
 
 // first pixel of tile t (block tiles: image b, rows 16 rb .., columns 8 cb ..)
 __device__ __forceinline__ long long shift_tile_v0(const ShiftP& p, int t, int& b, int& r0, int& c0) {
@@ -551,14 +560,150 @@ __device__ __forceinline__ bool shift_tile_live(const ShiftP& p, int t) {
     return (int)((v0 - b0 * hw) / (unsigned)p.W) < p.OH;
 }
 
+// Tap pairs j0 .. j0 + L - 1 of a half's chain: one m64nNk16 wgmma each, committed as one group.  A: the stage's half at
+// 16-byte unit a16, shifted per pair (tap_tab: shift | lbo << 16); B: the pair's weight rows, b_pair units apart.
+template <int N, int L>
+__device__ __forceinline__ void shift_chain(float* acc, const uint32_t* tap_tab, uint64_t ad_t, uint32_t a16, uint64_t bd, uint32_t b_pair,
+                                            int j0) {
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < L; ++k) {
+        const uint32_t e = tap_tab[j0 + k];
+        const uint64_t ad = ad_t | (uint64_t)((a16 + (e & 0xFFFFu)) & 0x3FFFu) | ((uint64_t)((e >> 16) & 0x3FFFu) << 16);
+        wgmma_c<N, 0, 0>(acc, ad, bd + (uint64_t)(j0 + k) * b_pair, j0 + k != 0);
+    }
+    wg_commit();
+}
+// the whole chain of a half (n_pairs tap pairs, in blocks of up to 4), drained
+template <int N>
+__device__ __forceinline__ void shift_half_mma(float* acc, const uint32_t* tap_tab, uint64_t ad_t, uint32_t a16, uint64_t bd, uint32_t b_pair,
+                                               int n_pairs) {
+    for (int j0 = 0; j0 < n_pairs; j0 += 4) {
+        switch (min(4, n_pairs - j0)) {
+            case 4: shift_chain<N, 4>(acc, tap_tab, ad_t, a16, bd, b_pair, j0); break;
+            case 3: shift_chain<N, 3>(acc, tap_tab, ad_t, a16, bd, b_pair, j0); break;
+            case 2: shift_chain<N, 2>(acc, tap_tab, ad_t, a16, bd, b_pair, j0); break;
+            default: shift_chain<N, 1>(acc, tap_tab, ad_t, a16, bd, b_pair, j0); break;
+        }
+    }
+    wg_wait_all();
+    wg_fence_regs<N / 2>(acc);
+}
+// fragments of D[64 x N] into rows row0 .. row0 + 63, columns col0 .. col0 + N - 1 of the accumulator tile
+template <int N>
+__device__ __forceinline__ void shift_acc_store(const float* acc, const AccTile& t, int row0, int col0) {
+    const int wt = threadIdx.x & 127, l = wt & 31;
+    float* r0 = t.p + (size_t)(row0 + 16 * (wt >> 5) + (l >> 2)) * t.stride + col0 + 2 * (l & 3);
+    float* r1 = r0 + 8 * t.stride;
+#pragma unroll
+    for (int i = 0; i < N / 8; ++i) {
+        *reinterpret_cast<float2*>(r0 + 8 * i) = make_float2(acc[4 * i], acc[4 * i + 1]);
+        *reinterpret_cast<float2*>(r1 + 8 * i) = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+    }
+}
+
+// column passes of k_conv_shift's MMA warpgroup for an accumulator width of nc (a multiple of 16): the fewest equal passes of
+// at most SH_MAX_N1 columns, each a multiple of 8
+__host__ __device__ constexpr int shift_passes(int nc) {
+    int np = 1;
+    while (nc / np > SH_MAX_N1 || nc % (8 * np) != 0) ++np;
+    return np;
+}
+
+// the MMA warpgroup's bulk copy of the next live tile from t_ld on into A stage s (the ring is filled in the order it is
+// consumed); the first warp of the warpgroup (loader) issues it
+__device__ __forceinline__ void shift_load_next(const ShiftP& p, uint32_t a_base, uint32_t a_full, int s, bool loader, int& t_ld) {
+    while (t_ld < p.n_tiles && !shift_tile_live(p, t_ld)) t_ld += gridDim.x;
+    if (t_ld >= p.n_tiles) return;
+    if (loader) {
+        int tb, tr0, tc0;
+        const long long v0 = shift_tile_v0(p, t_ld, tb, tr0, tc0);
+        long long px = p.total_pixels - v0;
+        if (px > p.a_pixels) px = p.a_pixels;
+        const uint32_t bytes = (uint32_t)px * 16u;
+        if (elect_one_sync()) {
+            mbar_arrive_expect_tx(a_full + 8 * s, bytes);
+            bulk_g2s(a_base + (uint32_t)s * p.a_stage, p.xp + v0 * 8, bytes, a_full + 8 * s);
+        }
+        __syncwarp();
+    }
+    t_ld += gridDim.x;
+}
+
+// MMA warpgroup h (0 / 1) of k_conv_shift for an accumulator width of NC columns (n_mma), in column passes of at most
+// SH_MAX_N1: per live tile, the chain over rows 64 h .. 64 h + 63 of the resident operands, then -- once the half's epilogue
+// warps have released it (acc_empty[h]) -- the fragments into those rows of the accumulator tile and an arrival on
+// acc_full[h].  The two warpgroups run side by side, each up to a tile ahead of its half's epilogue warps.  The first warp
+// of warpgroup 0 also issues the bulk copies: the weights once, then the A ring, refilling a stage once both chains that
+// read it have completed (its own, and warpgroup 1's arrival on a_empty).  Returns a nonzero abort code when a barrier
+// wait times out.
+template <int NC>
+__device__ __forceinline__ uint32_t shift_mma_role(const ShiftP& p, int h, uint32_t a_base, uint32_t b_base, uint32_t a_full,
+                                                   uint32_t a_empty, uint32_t b_full, uint32_t acc_full, uint32_t acc_empty,
+                                                   const uint32_t* tap_tab, const AccTile& acc_tile, volatile uint32_t* abort_g) {
+    static_assert(SH_STAGES == 2, "k_conv_shift: stage and phase are derived from the tile count");
+    constexpr int NP = shift_passes(NC), N = NC / NP;                 // NP passes of N columns
+    const bool first_warp = (threadIdx.x & 127) < 32, loader = h == 0 && first_warp;
+    if (loader) {
+        if (elect_one_sync()) {
+            mbar_arrive_expect_tx(b_full, (uint32_t)p.b_bytes);
+            bulk_g2s(b_base, p.wp, (uint32_t)p.b_bytes, b_full);
+        }
+        __syncwarp();
+    }
+    // live tile i of the CTA uses stage i % 2 in phase (i / 2) % 2: nothing else about the ring is kept in registers, which the
+    // chain needs; t_ld is the next live tile to load
+    int t_ld = blockIdx.x;
+    if (loader) {
+        shift_load_next(p, a_base, a_full, 0, true, t_ld);
+        shift_load_next(p, a_base, a_full, 1, true, t_ld);
+    }
+    if (!mbar_wait(b_full, 0)) return 2;
+    const uint64_t bd0 = gmma_desc_none(b_base, (uint32_t)NC, 8u);
+    const uint64_t ad_t = gmma_desc_none(0u, 0u, (uint32_t)p.sbo_units);     // A template: start address and LBO vary per tap pair
+    const uint32_t b_pair = 2u * NC;
+    int i = 0;
+    for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
+        if (!shift_tile_live(p, t)) continue;
+        const int s = i & 1;
+        const uint32_t ph = ((uint32_t)i >> 1) & 1u;
+        if (!mbar_wait(a_full + 8 * s, ph)) return 4;
+        if (*abort_g) return 0;
+        if (loader && (threadIdx.x & 31) == 0) shift_dbg(p, i, 0);
+        const uint32_t a16h = ((a_base + (uint32_t)s * p.a_stage) >> 4) + (uint32_t)h * 8u * (uint32_t)p.sbo_units;   // + 8 row groups
+#pragma unroll
+        for (int c = 0; c < NP; ++c) {
+            float acc[N / 2];
+            shift_half_mma<N>(acc, tap_tab, ad_t, a16h, bd0 + (uint64_t)(c * N), b_pair, p.n_pairs);
+            if (c == NP - 1) {          // this warpgroup's chains over stage s have completed
+                if (h == 1) {
+                    if (first_warp && elect_one_sync()) mbar_arrive(a_empty + 8 * s);
+                    __syncwarp();
+                } else if (loader) {    // refill stage s once warpgroup 1 is done with it too
+                    if (!mbar_wait(a_empty + 8 * s, ph)) return 8;
+                    shift_load_next(p, a_base, a_full, s, true, t_ld);
+                }
+            }
+            if (c == 0 && !mbar_wait(acc_empty + 8 * h, ((uint32_t)i & 1u) ^ 1u)) return 6;
+            shift_acc_store<N>(acc, acc_tile, 64 * h, c * N);
+        }
+        __syncwarp();
+        if (elect_one_sync()) mbar_arrive(acc_full + 8 * h);
+        __syncwarp();
+        if (first_warp && (threadIdx.x & 31) == 0) shift_dbg(p, i, 1 + h);
+        ++i;
+    }
+    return 0;
+}
+
 // MODE: 0 plain, 1 noisy (Philox z), 2 noisy with injected z (parity hook); SH_EPI_WARPS: epilogue warps, a
 // multiple of 4 and at least 8 (one quarter of the tile rows per warp % 4)
 template <int MODE, int SH_EPI_WARPS, bool POOL>
-__global__ void __launch_bounds__((1 + SH_EPI_WARPS) * 32, 1)
+__global__ void __launch_bounds__((SH_EPI_WARPS + 8) * 32, 1)
 k_conv_shift(const ShiftP p) {
     constexpr bool NOISY = MODE != 0;
-    constexpr int SH_THREADS = (1 + SH_EPI_WARPS) * 32;
-    static_assert(SH_EPI_WARPS >= 8 && SH_EPI_WARPS % 4 == 0, "the first 8 epilogue warps are the MMA warpgroups");
+    constexpr int SH_THREADS = (SH_EPI_WARPS + 8) * 32;      // epilogue warps, then the two MMA warpgroups
+    static_assert(SH_EPI_WARPS >= 8 && SH_EPI_WARPS % 4 == 0, "the MMA warpgroups start on a warpgroup boundary");
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 127u) & ~127u;
     const uint32_t b_base = base;
@@ -566,7 +711,8 @@ k_conv_shift(const ShiftP p) {
     const uint32_t bar_base = a_base + (uint32_t)SH_STAGES * (uint32_t)p.a_stage;
     const uint32_t a_full = bar_base, a_empty = bar_base + 8u * SH_STAGES;
     const uint32_t b_full = bar_base + 16u * SH_STAGES;
-    const uint32_t abort_slot = b_full + 8u, tab_slot = abort_slot + 4u;
+    const uint32_t acc_full = b_full + 8u, acc_empty = acc_full + 16u;          // per accumulator half
+    const uint32_t abort_slot = acc_empty + 16u, tab_slot = abort_slot + 4u;
     const uint32_t pool_slot = (tab_slot + 4u * SH_MAX_PAIRS + 15u) & ~15u;      // pooling exchange: [warp pair][2][8][16] floats
     const uint32_t acc_slot = pool_slot + 12u * 1024u;                            // accumulator tile: 128 rows x (n_mma + 4) floats
     uint8_t* gen0 = smem_raw + (base - smem_u32(smem_raw));
@@ -583,8 +729,12 @@ k_conv_shift(const ShiftP p) {
         tap_tab[tid] = (uint32_t)sh0 | ((uint32_t)(sh1 - sh0) << 16);
     }
     if (tid == 0) {
-        for (int s = 0; s < SH_STAGES; ++s) { mbar_init(a_full + 8 * s, 1); mbar_init(a_empty + 8 * s, 2); }
+        for (int s = 0; s < SH_STAGES; ++s) { mbar_init(a_full + 8 * s, 1); mbar_init(a_empty + 8 * s, 1); }
         mbar_init(b_full, 1);
+        for (int h = 0; h < 2; ++h) {
+            mbar_init(acc_full + 8 * h, 4);                         // the MMA warps
+            mbar_init(acc_empty + 8 * h, SH_EPI_WARPS / 2);         // the epilogue warps that read the half
+        }
         *abort_g = 0;
         fence_mbar_init();
     }
@@ -598,42 +748,28 @@ k_conv_shift(const ShiftP p) {
     __syncthreads();
     const int hw = p.H * p.W;
 
-    // loader: the whole warp walks the tiles (warp-uniform control flow), one elected lane issues the single-thread
-    // instructions (nn_wgmma.cuh: elect_one_sync)
-    if (warp == SH_EPI_WARPS) {
-        if (elect_one_sync()) {
-            mbar_arrive_expect_tx(b_full, (uint32_t)p.b_bytes);
-            bulk_g2s(b_base, p.wp, (uint32_t)p.b_bytes, b_full);
+    // role loops run on whole warps with warp-uniform control flow; one elected lane issues the single-thread instructions
+    // (nn_wgmma.cuh: elect_one_sync)
+    if (warp >= SH_EPI_WARPS) {
+        // ---- MMA warpgroups (one per accumulator half): the chain width is fixed once per launch (every n_mma the shift plan
+        // can produce)
+        const int h = (warp - SH_EPI_WARPS) >> 2;
+        uint32_t fail = 0;
+#define NN_SHIFT_MMA(NC)                                                                                                         \
+    case NC:                                                                                                                     \
+        fail = shift_mma_role<NC>(p, h, a_base, b_base, a_full, a_empty, b_full, acc_full, acc_empty, tap_tab, acc_tile, abort_g); \
+        break
+        switch (p.n_mma) {
+            NN_SHIFT_MMA(16); NN_SHIFT_MMA(32); NN_SHIFT_MMA(48); NN_SHIFT_MMA(64); NN_SHIFT_MMA(80); NN_SHIFT_MMA(96);
+            NN_SHIFT_MMA(112); NN_SHIFT_MMA(128); NN_SHIFT_MMA(144); NN_SHIFT_MMA(160); NN_SHIFT_MMA(176); NN_SHIFT_MMA(192);
+            NN_SHIFT_MMA(208); NN_SHIFT_MMA(224); NN_SHIFT_MMA(240); NN_SHIFT_MMA(256);
+            default: fail = 7; break;
         }
-        __syncwarp();
-        int s = 0;
-        uint32_t ph = 1u;
-        for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
-            if (!shift_tile_live(p, t)) continue;
-            if (!mbar_wait(a_empty + 8 * s, ph)) { *abort_g = 1; break; }
-            if (*abort_g) break;
-            int tb, tr0, tc0;
-            const long long v0 = shift_tile_v0(p, t, tb, tr0, tc0);
-            long long px = p.total_pixels - v0;
-            if (px > p.a_pixels) px = p.a_pixels;
-            const uint32_t bytes = (uint32_t)px * 16u;
-            if (elect_one_sync()) {
-                mbar_arrive_expect_tx(a_full + 8 * s, bytes);
-                bulk_g2s(a_base + (uint32_t)s * p.a_stage, p.xp + v0 * 8, bytes, a_full + 8 * s);
-            }
-            __syncwarp();
-            if (++s == SH_STAGES) { s = 0; ph ^= 1u; }
-        }
+#undef NN_SHIFT_MMA
+        if (fail) *abort_g = fail;
     } else {
-        // ---- MMA warpgroups (warps 0-7): the tile's accumulators, 64 columns at a time over the resident operands
-        const bool mma_wg = warp < 8;
-        const int wg = warp >> 2;
-        if (mma_wg && !mbar_wait(b_full, 0)) *abort_g = 2;
-        int s = 0;
-        uint32_t ph = 0u;
-        const uint64_t bd0 = gmma_desc_none(b_base, (uint32_t)p.n_mma, 8u);
-        const uint64_t ad_t = gmma_desc_none(0u, 0u, (uint32_t)p.sbo_units);   // A template: start address and LBO vary per tap pair
-        const int q = warp & 3, jq = warp >> 2;
+        // ---- epilogue warps: a warp reads the rows of one accumulator half
+        const int q = warp & 3, jq = warp >> 2, h = q >> 1;
         constexpr int per_q = SH_EPI_WARPS / 4;
         const int ohw = p.OH * p.OW;
         const int ngrp = (p.Cout + 3) >> 2;
@@ -645,40 +781,13 @@ k_conv_shift(const ShiftP p) {
         float st1[SH_POOL_IT], st2[SH_POOL_IT];          // pooled launches: per-thread sums of the pooled values it finalized
 #pragma unroll
         for (int it = 0; it < SH_POOL_IT; ++it) { st1[it] = 0.f; st2[it] = 0.f; }
+        const bool stamp = lane == 0 && (warp == 0 || warp == 2);      // one warp per half (shift_dbg)
         int i = 0;
         for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
             if (!shift_tile_live(p, t)) continue;
-            if (mma_wg && !*abort_g) {
-                if (!mbar_wait(a_full + 8 * s, ph)) {
-                    *abort_g = 4;
-                } else {
-                    if (p.dbg && i < 32 && warp == 0 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 0] = clock64();
-                    const uint32_t a_s = a_base + (uint32_t)s * p.a_stage + (uint32_t)wg * 128u * (uint32_t)p.sbo_units;   // + 8 row groups
-                    for (int c = 0; 64 * c < p.n_mma; ++c) {
-                        const int n = min(64, p.n_mma - 64 * c);
-                        float acc[1][32];
-                        wg_fence();
-#pragma unroll 1
-                        for (int j = 0; j < p.n_pairs; ++j) {
-                            const uint32_t e = tap_tab[j];
-                            const uint64_t ad = ad_t | (uint64_t)(((a_s >> 4) + (e & 0xFFFFu)) & 0x3FFFu) | ((uint64_t)((e >> 16) & 0x3FFFu) << 16);
-                            wgmma_n<0, 0>(acc[0], ad, bd0 + (uint64_t)(2 * j * p.n_mma + 64 * c), n, j != 0);
-                        }
-                        wg_commit();
-                        wg_wait_all();
-                        wg_fence_regs<32>(acc[0]);
-                        wg_acc_store(acc, acc_tile, 64 * wg, 64 * c, n);
-                    }
-                    __syncwarp();
-                    if ((warp & 3) == 0 && elect_one_sync()) mbar_arrive(a_empty + 8 * s);     // the A stage may be refilled
-                    __syncwarp();
-                    if (p.dbg && i < 32 && warp == 0 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 1] = clock64();
-                }
-                if (++s == SH_STAGES) { s = 0; ph ^= 1u; }
-            }
-            named_bar_sync(1, SH_EPI_WARPS * 32);          // the tile's accumulators are in the shared-memory tile
+            if (!mbar_wait(acc_full + 8 * h, (uint32_t)i & 1u)) { *abort_g = 5; break; }     // this half's accumulators are in the tile
             if (*abort_g) break;
-            if (p.dbg && i < 32 && warp == 0 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 2] = clock64();
+            if (stamp) shift_dbg(p, i, 3 + 2 * h);
             int b, ih, iw;
             bool row_ok;
             if (p.blk) {        // block tile: tile row = 8 * (image row in tile) + column, so a warp holds 4 rows x 8 columns
@@ -851,8 +960,10 @@ k_conv_shift(const ShiftP p) {
                 if (g4b < ngrp) one_group(g4b);
             }
             }
-            named_bar_sync(1, SH_EPI_WARPS * 32);          // the accumulator tile may be overwritten
-            if (p.dbg && i < 32 && warp == 0 && lane == 0) p.dbg[((size_t)blockIdx.x * 32 + i) * 4 + 3] = clock64();
+            __syncwarp();
+            if (elect_one_sync()) mbar_arrive(acc_empty + 8 * h);        // this warp's rows of the half may be overwritten
+            __syncwarp();
+            if (stamp) shift_dbg(p, i, 4 + 2 * h);
             ++i;
         }
         if (POOL && p.stat_partial) {
@@ -1662,7 +1773,7 @@ static bool make_shift_plan(const nn_conv_geom& g, bool noisy, ShiftPlan* out) {
     sp.n_tiles = (int)(((int64_t)g.B * g.H * g.W + UM_BLOCK_M - 1) / UM_BLOCK_M);
     // (the A ring is sized for the block tiles of the pooled launches: 16 + KH - 1 image rows)
     const int a_stage_blk = pad_to(((15 + g.KH - 1) * g.W + 8 + (g.KW - 1) + 8) * 16, 128);
-    sp.smem_bytes = 128 + (size_t)sp.b_bytes + (size_t)SH_STAGES * (a_stage_blk > sp.a_stage ? a_stage_blk : sp.a_stage) + 16 * SH_STAGES + 64 +
+    sp.smem_bytes = 128 + (size_t)sp.b_bytes + (size_t)SH_STAGES * (a_stage_blk > sp.a_stage ? a_stage_blk : sp.a_stage) + 16 * SH_STAGES + 96 +
                     4 * SH_MAX_PAIRS + 16 + 12 * 1024 + (size_t)UM_BLOCK_M * (sp.n_mma + 4) * 4;
     if (sp.n_pairs > SH_MAX_PAIRS) return false;
     sp.wp_bytes = (size_t)sp.b_bytes;
@@ -1944,7 +2055,7 @@ static int shift_conv_fwd(const nn_conv_fwd_args* a, const ShiftPlan& sp, int de
     const bool want_dbg = false;
 #endif
     if (want_dbg) {
-        const size_t rows = (size_t)grid * 16;           // 32 tiles x 4 stamps = 16 rows of 8
+        const size_t rows = (size_t)grid * 32 * SH_DBG / 8;      // 32 tiles x SH_DBG stamps, in rows of 8
         if (rows > g_dbg_ctas) {
             if (g_dbg_buf) cudaFree(g_dbg_buf);
             cudaMalloc(&g_dbg_buf, rows * 8 * sizeof(long long));
@@ -1964,7 +2075,7 @@ static int shift_conv_fwd(const nn_conv_fwd_args* a, const ShiftPlan& sp, int de
         NN_ONCE_PER_DEVICE({ \
             NN_CUDA_OK(cudaFuncSetAttribute(k_conv_shift<MODE, EW, POOL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
         });                                                                                                              \
-        k_conv_shift<MODE, EW, POOL><<<grid, (1 + EW) * 32, sp.smem_bytes, st>>>(p);                                    \
+        k_conv_shift<MODE, EW, POOL><<<grid, (EW + 8) * 32, sp.smem_bytes, st>>>(p);                                    \
     } while (0)
     if (p.pooled) {
         if (mode == 0) NN_SHIFT_LAUNCH(0, 16, true); else if (mode == 1) NN_SHIFT_LAUNCH(1, 16, true); else NN_SHIFT_LAUNCH(2, 16, true);
