@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define NN_ABI_VERSION 15
+#define NN_ABI_VERSION 16
 
 /* ---- common ---------------------------------------------------------------------- */
 
@@ -331,6 +331,14 @@ typedef struct nn_stage_args {
                                  nothing (noisynet.py:1560-1567); the caller passes stochastic = 0 (hardware_model.py:283-286) */
     int32_t stats_ready;      /* 1: mean / invstd (and the running statistics, and *xmax_out = 0) were already produced by
                                  the conv launch (nn_conv_fwd_args.bn_mean): skip the statistics pass (pool must be 0)  */
+    double drop_p;            /* dropout rate in [0, 1), 0 = off: nn.Dropout(p) after ReLU + clamp and before the next
+                                 quantizer (noisynet.py:375-376, :456-457, :512-513, :565-566); the quantizer and act /
+                                 xmax_out see x * mask / (1 - p).  0 in eval (dropout is the identity there)             */
+    uint8_t* keep;            /* out [B,C,H',W'] uint8 keep mask (1 = kept), the BN input's layout like argmax; required
+                                 when drop_p > 0, read back by nn_stage_bwd                                               */
+    const uint8_t* keep_inject; /* optional mask in the layout of `keep`, read instead of the Philox draw (parity hook)   */
+    nn_rng drop_rng;          /* the keep decisions' own Philox stream: element (pixel, channel c) draws group
+                                 2 * (pixel * Cp/8 + c/8) + (c%8)/4, word c%4, and is kept iff u01 >= (float)drop_p     */
 } nn_stage_args;
 int64_t nn_stage_scratch_bytes(int C);
 int nn_stage_fwd(const nn_stage_args* a, int device, void* stream);
@@ -353,6 +361,9 @@ typedef struct nn_stage_bwd_args {
                                  pixel grid (the producing conv's INPUT grid, see nn_conv_wgrad_args); the buffer
                                  must have been zeroed once -- only output positions are ever written            */
     int32_t virt_H, virt_W;
+    double drop_p;            /* dropout rate of the forward (noisynet.py:456-457, :512-513, :565-566), 0 = off:
+                                 g * mask / (1 - p), and the quantizer STE tests the dropped and scaled value             */
+    const uint8_t* keep;      /* the forward's keep mask (nn_stage_args.keep), required when drop_p > 0               */
 } nn_stage_bwd_args;
 int nn_stage_bwd(const nn_stage_bwd_args* a, int device, void* stream);
 

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("NN_LIB_PATH") or os.path.join(_HERE, "lib", "libnoisynet_b200.so")   # NN_LIB_PATH: instrumented debug builds
-ABI_VERSION = 15
+ABI_VERSION = 16
 
 NOISE_NONE, NOISE_MERGED, NOISE_EXTERNAL = 0, 1, 2
 PREC_FP32, PREC_TF32, PREC_BF16 = 0, 1, 2
@@ -85,7 +85,8 @@ class StageArgs(C.Structure):
                 ("act_max", C.c_float), ("q_bits", C.c_int32), ("q_hi", C.c_double), ("stochastic", C.c_float),
                 ("u_inject", C.c_void_p), ("rng", Rng), ("xp", C.c_void_p), ("Cp", C.c_int32),
                 ("act", C.c_void_p), ("xmax_out", C.c_void_p), ("scratch", C.c_void_p), ("eval_mode", C.c_int32),
-                ("stats_ready", C.c_int32)]
+                ("stats_ready", C.c_int32), ("drop_p", C.c_double), ("keep", C.c_void_p), ("keep_inject", C.c_void_p),
+                ("drop_rng", Rng)]
 
 
 class StageBwdArgs(C.Structure):
@@ -95,7 +96,8 @@ class StageBwdArgs(C.Structure):
                 ("act_max", C.c_float), ("q_bits", C.c_int32), ("q_hi", C.c_double),
                 ("dgamma", C.c_void_p), ("dbeta", C.c_void_p), ("gyp", C.c_void_p), ("Cp", C.c_int32),
                 ("gy_f32", C.c_void_p), ("scratch", C.c_void_p),
-                ("gy_layout", C.c_int32), ("virt_H", C.c_int32), ("virt_W", C.c_int32)]
+                ("gy_layout", C.c_int32), ("virt_H", C.c_int32), ("virt_W", C.c_int32),
+                ("drop_p", C.c_double), ("keep", C.c_void_p)]
 
 
 class TailArgs(C.Structure):

@@ -156,11 +156,35 @@ struct BnActP {
     float act_max, q_scale, q_max, stoch;
     int quant;
     nn_rng rng;
+    // dropout (DROP instantiations only): keep mask out [B,C,HW] uint8, optional injected mask, rate, 1/(1-p), stream
+    uint8_t* keep;
+    const uint8_t* keep_inject;
+    float drop_p, drop_k;
+    nn_rng drop_rng;
 };
 
+// Dropout between the clamp and the quantizer (noisynet.py:456, :512, :565): torch's x * (bernoulli(1-p) / (1-p)) in fp32,
+// k = fl(1 / fl(1 - p)).  The keep decisions of a (pixel, 8-channel chunk) thread i come from their own Philox stream
+// (drop_rng): groups 2i and 2i + 1 -- the group indices of the rounding draws, so those stay the same draws whether dropout
+// is on or off -- word j for channel j of the chunk; keep iff u01 >= p.  The mask is stored (BN-input layout) for the backward.
+__device__ __forceinline__ float stage_drop(float v, bool keep, float k) { return keep ? __fmul_rn(v, k) : 0.f; }
+
+// keep bits of one (pixel, chunk) thread, bit j = channel j of the chunk (one register instead of eight words)
+__device__ __forceinline__ unsigned stage_keep_bits(const NnRng& ds, unsigned i, float p) {
+    const uint4 k0 = nn_philox(ds, (uint64_t)i * 2), k1 = nn_philox(ds, (uint64_t)i * 2 + 1);
+    const uint32_t kr[8] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z, k1.w};
+    unsigned bits = 0u;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) bits |= (nn_u01(kr[j]) >= p ? 1u : 0u) << j;
+    return bits;
+}
+
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 k_bn_act_pack(const BnActP p) {
     const NnRng rs = nn_rng_load(p.rng);
+    NnRng ds{};
+    if (DROP) ds = nn_rng_load(p.drop_rng);
     const int chunks = p.Cp >> 3;
     const unsigned npix = (unsigned)p.B * p.HW, total = npix * chunks;      // 32-bit index arithmetic
     float vmax = 0.f;
@@ -177,6 +201,12 @@ k_bn_act_pack(const BnActP p) {
             rnd[1] = nn_philox(rs, (uint64_t)i * 2 + 1);
         }
         const uint32_t* rr = reinterpret_cast<const uint32_t*>(rnd);
+        uint4 krnd[2];
+        if (DROP && !p.keep_inject) {
+            krnd[0] = nn_philox(ds, (uint64_t)i * 2);
+            krnd[1] = nn_philox(ds, (uint64_t)i * 2 + 1);
+        }
+        const uint32_t* kr = reinterpret_cast<const uint32_t*>(krnd);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const int c = chunk * 8 + j;
@@ -186,6 +216,11 @@ k_bn_act_pack(const BnActP p) {
                 float v = (__ldg(p.x + o) - __ldg(p.mean + c)) * __ldg(p.invstd + c) * __ldg(p.gamma + c) + __ldg(p.beta + c);
                 v = fmaxf(v, 0.f);                                          // ReLU
                 if (p.act_max > 0.f) v = fminf(v, p.act_max);               // clamp(max=act_max)
+                if (DROP) {
+                    const bool keep = p.keep_inject ? __ldg(p.keep_inject + o) != 0 : nn_u01(kr[j]) >= p.drop_p;
+                    p.keep[o] = (uint8_t)keep;
+                    v = stage_drop(v, keep, p.drop_k);
+                }
                 float val = v;
                 if (p.quant) {
                     const float u = p.stoch > 0.f ? (p.u_inject ? __ldg(p.u_inject + o) : nn_usym(rr[j], p.stoch)) : 0.f;
@@ -211,9 +246,12 @@ k_bn_act_pack(const BnActP p) {
 // no fp32 copy): same thread mapping and arithmetic, but the run-time option checks are compiled out and the index
 // arithmetic is 32-bit.  Registers are capped for 6 blocks/SM: the kernel is latency-bound, occupancy matters more
 // than instruction count (variants that kept parameters in registers were slower).
-__global__ void __launch_bounds__(256, 6)
+template <bool DROP>
+__global__ void __launch_bounds__(256, DROP ? 5 : 6)      // the keep bits need a few registers more than 6 blocks leave
 k_bn_act_pack_lean(const BnActP p) {
     const NnRng rs = nn_rng_load(p.rng);
+    NnRng ds{};
+    if (DROP) ds = nn_rng_load(p.drop_rng);
     const unsigned chunks = (unsigned)(p.Cp >> 3), HW = (unsigned)p.HW, C = (unsigned)p.C;
     const unsigned npix = (unsigned)p.B * HW, total = npix * chunks;
     const float act_hi = p.act_max > 0.f ? p.act_max : __int_as_float(0x7f800000);
@@ -224,6 +262,7 @@ k_bn_act_pack_lean(const BnActP p) {
         const unsigned b = pixel / HW, r = pixel - b * HW;
         const unsigned c0 = chunk * 8;
         const float* src = p.x + (b * C + c0) * HW + r;           // element index < 2^31 (host check)
+        const unsigned kbits = DROP ? stage_keep_bits(ds, i, p.drop_p) : 0u;     // before the rounding words are live
         const uint4 r0 = nn_philox(rs, (uint64_t)i * 2), r1 = nn_philox(rs, (uint64_t)i * 2 + 1);
         const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
         __align__(16) __nv_bfloat16 out[8];
@@ -234,6 +273,11 @@ k_bn_act_pack_lean(const BnActP p) {
             if (c < C) {
                 float v = (__ldg(src + j * HW) - __ldg(p.mean + c)) * __ldg(p.invstd + c) * __ldg(p.gamma + c) + __ldg(p.beta + c);
                 v = fminf(fmaxf(v, 0.f), act_hi);                                   // ReLU, clamp(max=act_max)
+                if (DROP) {
+                    const bool keep = (kbits >> j) & 1u;
+                    p.keep[(b * C + c0) * HW + r + j * HW] = (uint8_t)keep;
+                    v = stage_drop(v, keep, p.drop_k);
+                }
                 const float u = __fadd_rn(__fmul_rn(nn_u01(rr[j]), two_s), -stoch);    // == nn_usym(rr[j], stoch)
                 code = quant_code(v, q_scale, q_max, u);
                 vmax = fmaxf(vmax, __fmul_rn(code, q_scale));
@@ -253,10 +297,13 @@ k_bn_act_pack_lean(const BnActP p) {
 // consecutive pixels: lane = pixel, so every channel read is one 128-byte line of the NCHW input (the chunk-fastest
 // mapping touched 32 different lines per load instruction); the codes are staged in shared memory as the tile's NHWC
 // image and leave as one contiguous 32 x Cp x 2 byte run.  Measured at batch 512, 65 channels 14x14: 43.5 -> see DESIGN.
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 k_bn_act_pack_tiled(const BnActP p) {
     extern __shared__ uint4 s_tile[];                       // [32 pixels][pitch] 16-byte chunks
     const NnRng rs = nn_rng_load(p.rng);
+    NnRng ds{};
+    if (DROP) ds = nn_rng_load(p.drop_rng);
     const unsigned chunks = (unsigned)(p.Cp >> 3), HW = (unsigned)p.HW, C = (unsigned)p.C;
     const unsigned pitch = chunks | 1u;                      // odd pitch: conflict-free 16-byte column writes
     const unsigned npix = (unsigned)p.B * HW;
@@ -274,6 +321,7 @@ k_bn_act_pack_tiled(const BnActP p) {
             if (pix_ok) {
                 const unsigned i = pixel * chunks + chunk;
                 const float* src = p.x + (b * C + c0) * HW + r;           // element index < 2^31 (host check)
+                const unsigned kbits = DROP ? stage_keep_bits(ds, i, p.drop_p) : 0u;
                 const uint4 r0 = nn_philox(rs, (uint64_t)i * 2), r1 = nn_philox(rs, (uint64_t)i * 2 + 1);
                 const uint32_t rr[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
 #pragma unroll
@@ -283,6 +331,11 @@ k_bn_act_pack_tiled(const BnActP p) {
                     if (c < C) {
                         float v = (__ldg(src + j * HW) - __ldg(p.mean + c)) * __ldg(p.invstd + c) * __ldg(p.gamma + c) + __ldg(p.beta + c);
                         v = fminf(fmaxf(v, 0.f), act_hi);                                   // ReLU, clamp(max=act_max)
+                        if (DROP) {
+                            const bool keep = (kbits >> j) & 1u;
+                            p.keep[(b * C + c0) * HW + r + j * HW] = (uint8_t)keep;      // lane = pixel: 32 consecutive bytes
+                            v = stage_drop(v, keep, p.drop_k);
+                        }
                         const float u = __fadd_rn(__fmul_rn(nn_u01(rr[j]), two_s), -stoch);    // == nn_usym(rr[j], stoch)
                         code = quant_code(v, q_scale, q_max, u);
                         vmax = fmaxf(vmax, __fmul_rn(code, q_scale));
@@ -315,19 +368,29 @@ struct BnBwdP {
     float *dbeta, *dgamma;        // written by the last slice's block of each channel
     int B, C, HW;
     float act_max, q_hi;
+    const uint8_t* keep;          // dropout mask of the forward (DROP instantiations only), BN-input layout
+    float drop_k;                 // 1 / (1 - p)
 };
 
+template <bool DROP>
 __device__ __forceinline__ float stage_dv(float g, float x, float mean, float invstd, float gamma, float beta,
-                                          float act_max, float q_hi, float& xhat) {
+                                          float act_max, float q_hi, float& xhat, bool keep = true, float k = 1.f) {
     xhat = (x - mean) * invstd;
     const float v = xhat * gamma + beta;
     // ReLU: v > 0; clamp(max): v <= act_max; quantizer STE (hardware_model.py:176-183): 0 <= clamped <= q_hi
     bool pass = v > 0.f;
     if (act_max > 0.f) pass = pass && (v <= act_max);
+    if (DROP) {
+        // dropout: the quantizer saw fl(clamped * k) and the gradient is fl(g * k) on kept elements, 0 on dropped ones
+        pass = pass && keep;
+        if (q_hi > 0.f) pass = pass && (__fmul_rn(fminf(v, act_max > 0.f ? act_max : v), k) <= q_hi);
+        return pass ? __fmul_rn(g, k) : 0.f;
+    }
     if (q_hi > 0.f) pass = pass && (fminf(v, act_max > 0.f ? act_max : v) <= q_hi);
     return pass ? g : 0.f;
 }
 
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 k_bn_bwd_stats(const BnBwdP p) {
     const int c = blockIdx.x, sp = blockIdx.y;
@@ -340,17 +403,19 @@ k_bn_bwd_stats(const BnBwdP p) {
     unsigned i = threadIdx.x;
     for (; i + 3 * blockDim.x < (unsigned)n; i += 4 * blockDim.x) {         // eight loads in flight, sums in element order
         float gv[4], xv[4];
+        bool kv[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             const int64_t o = ((int64_t)(b0 + (int)bi) * p.C + c) * p.HW + r;
             gv[k] = __ldg(p.g + o); xv[k] = __ldg(p.x + o);
+            kv[k] = DROP ? __ldg(p.keep + o) != 0 : true;
             bi += step_b; r += step_r;
             if (r >= (unsigned)p.HW) { r -= (unsigned)p.HW; ++bi; }
         }
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             float xhat;
-            const float dv = stage_dv(gv[k], xv[k], mean, invstd, gamma, beta, p.act_max, p.q_hi, xhat);
+            const float dv = stage_dv<DROP>(gv[k], xv[k], mean, invstd, gamma, beta, p.act_max, p.q_hi, xhat, kv[k], p.drop_k);
             s1 += dv; s2 += (double)dv * xhat;
         }
     }
@@ -358,7 +423,8 @@ k_bn_bwd_stats(const BnBwdP p) {
         const int b = b0 + (int)bi;
         const int64_t o = ((int64_t)b * p.C + c) * p.HW + r;
         float xhat;
-        const float dv = stage_dv(__ldg(p.g + o), __ldg(p.x + o), mean, invstd, gamma, beta, p.act_max, p.q_hi, xhat);
+        const float dv = stage_dv<DROP>(__ldg(p.g + o), __ldg(p.x + o), mean, invstd, gamma, beta, p.act_max, p.q_hi, xhat,
+                                        DROP ? __ldg(p.keep + o) != 0 : true, p.drop_k);
         s1 += dv; s2 += (double)dv * xhat;
         bi += step_b; r += step_r;
         if (r >= (unsigned)p.HW) { r -= (unsigned)p.HW; ++bi; }
@@ -393,8 +459,11 @@ struct BnBwdApplyP {
     float act_max, q_hi, inv_count;
     int planes, vH, vW;           // planes = 1: output in the planes layout [chunk][plane_stride][8] on a vH x vW grid
     long long plane_stride;
+    const uint8_t* keep;          // dropout mask (DROP instantiations only), read at the index of g and x
+    float drop_k;
 };
 
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 k_bn_bwd_apply(const BnBwdApplyP p) {
     // one thread = (pooled pixel, 8-channel chunk): the BN-backward value of each channel is computed ONCE and
@@ -421,8 +490,8 @@ k_bn_bwd_apply(const BnBwdApplyP p) {
                 const size_t o = ((size_t)b * p.C + c) * PHW + r;
                 float xhat;
                 const float invstd = __ldg(p.invstd + c), gamma = __ldg(p.gamma + c);
-                const float dv = stage_dv(__ldg(p.g + o), __ldg(p.x + o), __ldg(p.mean + c), invstd, gamma,
-                                          __ldg(p.beta + c), p.act_max, p.q_hi, xhat);
+                const float dv = stage_dv<DROP>(__ldg(p.g + o), __ldg(p.x + o), __ldg(p.mean + c), invstd, gamma,
+                                                __ldg(p.beta + c), p.act_max, p.q_hi, xhat, DROP ? __ldg(p.keep + o) != 0 : true, p.drop_k);
                 d[j] = gamma * invstd * (dv - __ldg(p.dbeta + c) * p.inv_count - xhat * __ldg(p.dgamma + c) * p.inv_count);
                 pos[j] = p.pool ? (int)__ldg(p.amax + o) : 0;
             }
@@ -448,7 +517,7 @@ k_bn_bwd_apply(const BnBwdApplyP p) {
 
 // Hot-path variant of k_bn_bwd_apply: same thread mapping and arithmetic; pooling and the output layout are
 // compile-time, no fp32 copy, 32-bit indices, registers capped for occupancy (see k_bn_act_pack_lean).
-template <bool POOL, bool PLANES>
+template <bool POOL, bool PLANES, bool DROP>
 __global__ void __launch_bounds__(256, 5)
 k_bn_bwd_apply_lean(const BnBwdApplyP p) {
     const unsigned chunks = (unsigned)(p.Cp >> 3), C = (unsigned)p.C;
@@ -473,8 +542,8 @@ k_bn_bwd_apply_lean(const BnBwdApplyP p) {
                 const unsigned o = o0 + j * PHW;
                 float xhat;
                 const float invstd = __ldg(p.invstd + c), gamma = __ldg(p.gamma + c);
-                const float dv = stage_dv(__ldg(p.g + o), __ldg(p.x + o), __ldg(p.mean + c), invstd, gamma,
-                                          __ldg(p.beta + c), p.act_max, p.q_hi, xhat);
+                const float dv = stage_dv<DROP>(__ldg(p.g + o), __ldg(p.x + o), __ldg(p.mean + c), invstd, gamma,
+                                                __ldg(p.beta + c), p.act_max, p.q_hi, xhat, DROP ? __ldg(p.keep + o) != 0 : true, p.drop_k);
                 d[j] = gamma * invstd * (dv - __ldg(p.dbeta + c) * inv_count - xhat * __ldg(p.dgamma + c) * inv_count);
                 pos[j] = POOL ? (int)__ldg(p.amax + o) : 0;
             }
@@ -496,6 +565,7 @@ k_bn_bwd_apply_lean(const BnBwdApplyP p) {
 // argmax slices are CONTIGUOUS (C * PH * PW elements): thread t reads element t, t + 256, ... (the chunk-fastest mapping of
 // k_bn_bwd_apply_lean touched 32 cache lines per load instruction); the sample's NHWC bf16 gradient image (zeros included)
 // is assembled in shared memory and leaves as one contiguous run.  Same arithmetic as k_bn_bwd_apply.
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 k_bn_bwd_apply_img(const BnBwdApplyP p) {
     extern __shared__ uint4 s_img4[];
@@ -511,8 +581,8 @@ k_bn_bwd_apply_img(const BnBwdApplyP p) {
             const unsigned c = e / PHW, r = e - c * PHW, ph = r / PW, pw = r - ph * PW;
             float xhat;
             const float invstd = __ldg(p.invstd + c), gamma = __ldg(p.gamma + c);
-            const float dv = stage_dv(__ldg(p.g + o0 + e), __ldg(p.x + o0 + e), __ldg(p.mean + c), invstd, gamma, __ldg(p.beta + c),
-                                      p.act_max, p.q_hi, xhat);
+            const float dv = stage_dv<DROP>(__ldg(p.g + o0 + e), __ldg(p.x + o0 + e), __ldg(p.mean + c), invstd, gamma, __ldg(p.beta + c),
+                                            p.act_max, p.q_hi, xhat, DROP ? __ldg(p.keep + o0 + e) != 0 : true, p.drop_k);
             const float d = gamma * invstd * (dv - __ldg(p.dbeta + c) * inv_count - xhat * __ldg(p.dgamma + c) * inv_count);
             const unsigned pos = __ldg(p.amax + o0 + e);
             const unsigned oh = 2 * ph + (pos >> 1), ow = 2 * pw + (pos & 1);
@@ -1098,6 +1168,10 @@ extern "C" int nn_stage_fwd(const nn_stage_args* a, int device, void* stream) {
     if (a->pool && ((a->H | a->W) & 1)) return nn_fail("nn_stage_fwd: pooling needs even H, W%s", "");
     if (a->Cp % 8 || a->Cp < a->C) return nn_fail("nn_stage_fwd: bad Cp%s", "");
     if (a->eval_mode && (!a->running_mean || !a->running_var)) return nn_fail("nn_stage_fwd: eval_mode needs the running statistics%s", "");
+    if (!(a->drop_p >= 0.0 && a->drop_p < 1.0)) return nn_fail("nn_stage_fwd: drop_p must lie in [0, 1)%s", "");
+    const bool drop = a->drop_p > 0.0;
+    if (drop && !a->keep) return nn_fail("nn_stage_fwd: drop_p > 0 needs the keep mask buffer%s", "");
+    if (drop && a->eval_mode) return nn_fail("nn_stage_fwd: dropout is the identity in eval mode (pass drop_p = 0)%s", "");
     NN_SET_DEVICE(device);
     cudaStream_t st = (cudaStream_t)stream;
     const float* bn_in = a->in;
@@ -1136,22 +1210,32 @@ extern "C" int nn_stage_fwd(const nn_stage_args* a, int device, void* stream) {
     double scale = a->q_bits > 0 ? a->q_hi / qmax : 1.0;
     if (scale < 1e-6) scale = 1e-6;
     p.q_scale = (float)scale; p.q_max = (float)qmax; p.stoch = a->stochastic; p.rng = a->rng;
+    // dropout: k = fl(1 / fl(1 - p)) as torch forms bernoulli_(1 - p).div_(1 - p) on fp32 (noisynet.py:375-376)
+    p.keep = drop ? a->keep : nullptr; p.keep_inject = drop ? a->keep_inject : nullptr;
+    p.drop_p = (float)a->drop_p; p.drop_k = drop ? 1.0f / (float)(1.0 - a->drop_p) : 1.0f; p.drop_rng = a->drop_rng;
     const int64_t items = (int64_t)a->B * HW * (a->Cp / 8);
-    const bool lean = ST_CHUNK_FAST && p.quant && p.stoch > 0.f && !p.u_inject && !p.act &&
+    const bool lean = ST_CHUNK_FAST && p.quant && p.stoch > 0.f && !p.u_inject && !p.keep_inject && !p.act &&
                       (int64_t)a->B * a->C * HW < ((int64_t)1 << 31) && items < ((int64_t)1 << 31);
     const size_t tile_smem = (size_t)32 * ((a->Cp / 8) | 1) * 16;
     if (lean && HW >= 32 && tile_smem <= 48 * 1024) {
         const int64_t tiles = ((int64_t)a->B * HW + 31) / 32;
         const int64_t cap = (int64_t)nn_num_sms(device) * 16;
-        k_bn_act_pack_tiled<<<(int)(tiles < cap ? tiles : cap), 256, tile_smem, st>>>(p);
-    } else if (lean) k_bn_act_pack_lean<<<grid_cap(items, device), 256, 0, st>>>(p);
-    else k_bn_act_pack<<<grid_cap(items, device), 256, 0, st>>>(p);
+        if (drop) k_bn_act_pack_tiled<true><<<(int)(tiles < cap ? tiles : cap), 256, tile_smem, st>>>(p);
+        else k_bn_act_pack_tiled<false><<<(int)(tiles < cap ? tiles : cap), 256, tile_smem, st>>>(p);
+    } else if (lean) {
+        if (drop) k_bn_act_pack_lean<true><<<grid_cap(items, device), 256, 0, st>>>(p);
+        else k_bn_act_pack_lean<false><<<grid_cap(items, device), 256, 0, st>>>(p);
+    } else if (drop) k_bn_act_pack<true><<<grid_cap(items, device), 256, 0, st>>>(p);
+    else k_bn_act_pack<false><<<grid_cap(items, device), 256, 0, st>>>(p);
     NN_LAUNCH_OK();
     return 0;
 }
 
 extern "C" int nn_stage_bwd(const nn_stage_bwd_args* a, int device, void* stream) {
     if (!a || !a->g || !a->x || !a->gyp || !a->scratch) return nn_fail("nn_stage_bwd: null argument%s", "");
+    if (!(a->drop_p >= 0.0 && a->drop_p < 1.0)) return nn_fail("nn_stage_bwd: drop_p must lie in [0, 1)%s", "");
+    const bool drop = a->drop_p > 0.0;
+    if (drop && !a->keep) return nn_fail("nn_stage_bwd: drop_p > 0 needs the forward's keep mask%s", "");
     NN_SET_DEVICE(device);
     cudaStream_t st = (cudaStream_t)stream;
     const int PH = a->pool ? a->H / 2 : a->H, PW = a->pool ? a->W / 2 : a->W;
@@ -1160,15 +1244,18 @@ extern "C" int nn_stage_bwd(const nn_stage_bwd_args* a, int device, void* stream
     q.partial = (double*)a->scratch; q.counters = (unsigned*)(q.partial + (size_t)a->C * ST_SPLITS * 2);
     q.dbeta = a->dbeta; q.dgamma = a->dgamma; q.B = a->B; q.C = a->C; q.HW = PH * PW; q.act_max = a->act_max;
     q.q_hi = a->q_bits > 0 ? (float)a->q_hi : 0.f;
+    q.keep = drop ? a->keep : nullptr; q.drop_k = drop ? 1.0f / (float)(1.0 - a->drop_p) : 1.0f;
     const int splits = stage_splits((int64_t)a->B * PH * PW);
     dim3 grid(a->C, splits);
-    k_bn_bwd_stats<<<grid, 256, 0, st>>>(q);
+    if (drop) k_bn_bwd_stats<true><<<grid, 256, 0, st>>>(q);
+    else k_bn_bwd_stats<false><<<grid, 256, 0, st>>>(q);
     NN_LAUNCH_OK();
     BnBwdApplyP p;
     p.g = a->g; p.x = a->x; p.mean = a->mean; p.invstd = a->invstd; p.gamma = a->gamma; p.beta = a->beta;
     p.dbeta = a->dbeta; p.dgamma = a->dgamma; p.amax = a->argmax; p.gyp = (__nv_bfloat16*)a->gyp; p.gy_f32 = a->gy_f32;
     p.B = a->B; p.C = a->C; p.OH = a->H; p.OW = a->W; p.Cp = a->Cp; p.pool = a->pool;
     p.act_max = a->act_max; p.q_hi = q.q_hi; p.inv_count = 1.f / ((float)a->B * PH * PW);
+    p.keep = q.keep; p.drop_k = q.drop_k;
     if (a->pool && !a->argmax) return nn_fail("nn_stage_bwd: argmax missing%s", "");
     p.planes = a->gy_layout == NN_PACK_SHIFT ? 1 : 0;
     p.vH = p.vW = 0; p.plane_stride = 0;
@@ -1184,12 +1271,20 @@ extern "C" int nn_stage_bwd(const nn_stage_bwd_args* a, int device, void* stream
     const size_t img_bytes = (size_t)a->H * a->W * a->Cp * 2;
     if (lean && a->pool && !p.planes && img_bytes <= 48 * 1024 && PH * PW >= 16) {
         const int cap = nn_num_sms(device) * 8;
-        k_bn_bwd_apply_img<<<a->B < cap ? a->B : cap, 256, img_bytes, st>>>(p);
-    } else if (!lean) k_bn_bwd_apply<<<agrid, 256, 0, st>>>(p);
-    else if (a->pool && p.planes) k_bn_bwd_apply_lean<true, true><<<agrid, 256, 0, st>>>(p);
-    else if (a->pool) k_bn_bwd_apply_lean<true, false><<<agrid, 256, 0, st>>>(p);
-    else if (p.planes) k_bn_bwd_apply_lean<false, true><<<agrid, 256, 0, st>>>(p);
-    else k_bn_bwd_apply_lean<false, false><<<agrid, 256, 0, st>>>(p);
+        if (drop) k_bn_bwd_apply_img<true><<<a->B < cap ? a->B : cap, 256, img_bytes, st>>>(p);
+        else k_bn_bwd_apply_img<false><<<a->B < cap ? a->B : cap, 256, img_bytes, st>>>(p);
+    } else if (!lean) {
+        if (drop) k_bn_bwd_apply<true><<<agrid, 256, 0, st>>>(p);
+        else k_bn_bwd_apply<false><<<agrid, 256, 0, st>>>(p);
+    } else if (drop) {
+        if (a->pool && p.planes) k_bn_bwd_apply_lean<true, true, true><<<agrid, 256, 0, st>>>(p);
+        else if (a->pool) k_bn_bwd_apply_lean<true, false, true><<<agrid, 256, 0, st>>>(p);
+        else if (p.planes) k_bn_bwd_apply_lean<false, true, true><<<agrid, 256, 0, st>>>(p);
+        else k_bn_bwd_apply_lean<false, false, true><<<agrid, 256, 0, st>>>(p);
+    } else if (a->pool && p.planes) k_bn_bwd_apply_lean<true, true, false><<<agrid, 256, 0, st>>>(p);
+    else if (a->pool) k_bn_bwd_apply_lean<true, false, false><<<agrid, 256, 0, st>>>(p);
+    else if (p.planes) k_bn_bwd_apply_lean<false, true, false><<<agrid, 256, 0, st>>>(p);
+    else k_bn_bwd_apply_lean<false, false, false><<<agrid, 256, 0, st>>>(p);
     NN_LAUNCH_OK();
     return 0;
 }

@@ -1,18 +1,21 @@
 """NoisyNetEngine -- the whole CIFAR NoisyNet training step (noisynet.py:1276-1542) as an explicit schedule
 of this library's kernels, with static buffers (CUDA-graph capturable, no autograd, no torch kernels):
 
-  forward : input quantize+pack -> [tensor-core fused noisy conv -> pool+BN+ReLU+clamp+quantize+pack stage] x 2
-            -> [tensor-core fused noisy linear -> BN+ReLU+clamp+quantize+pack stage] -> fused noisy linear -> BN + CE head
-  backward: head -> wgrad/dgrad (tensor cores) -> stage backward (STE/clamp/ReLU masks, BN backward, pool routing,
+  forward : input quantize+pack -> [tensor-core fused noisy conv -> pool+BN+ReLU+clamp+dropout+quantize+pack stage] x 2
+            -> [tensor-core fused noisy linear -> BN+ReLU+clamp+dropout+quantize+pack stage] -> fused noisy linear -> BN + CE head
+  backward: head -> wgrad/dgrad (tensor cores) -> stage backward (STE/dropout/clamp/ReLU masks, BN backward, pool routing,
             emitted as NHWC bf16 for the next wgrad/dgrad) ... -> conv1 wgrad
   update  : [flat-gradient all-reduce] -> fused AdamW + weight clamp + max|W|
 
 Activations travel between layers as NHWC bf16 integer codes (exact 4-bit operands for the tensor cores);
 fp32 NCHW tensors exist only where the maths needs them (noisy conv outputs, pooled BN inputs, gradients).
 Parameters, BN buffers and quantizer ranges are those of a `NoisyNet` module (state_dict compatible).
-Requires q_a > 0 and q_w > 0 on every layer (per-layer bit widths and act_max1..3 are honoured); steady-state
-semantics (the i < 20 side statistics, bias, dropout and the alternative noise models are the module path's).
-``eval_forward`` is the model.eval() forward (running BN statistics, no stochastic rounding, noise still injected).
+Per-layer bit widths (q = 0: bf16 operands) and act_max1..3 are honoured; steady-state semantics (the i < 20 side
+statistics, bias and the alternative noise models are the module path's).  --dropout p (noisynet.py:375-376) runs inside
+the stage kernels at the reference's sites -- after relu2 and relu3, and after relu1 when --dropout_conv > 0 (at rate
+--dropout, as the reference does) -- with a Bernoulli keep mask drawn in the forward kernel and reused by the backward.
+``eval_forward`` is the model.eval() forward (running BN statistics, no stochastic rounding, no dropout, noise still
+injected).
 """
 import ctypes as C
 import os
@@ -44,9 +47,11 @@ class NoisyNetEngine:
             raise NotImplementedError("NoisyNetEngine: multiplicative weight noise (--n_w) is served by the module path")
         if max(self.q_w) > 7:
             raise ValueError("NoisyNetEngine: weight codes are int8 (q_w <= 7)")
-        if a.use_bias or a.dropout > 0 or a.dropout_conv > 0:
-            raise NotImplementedError("NoisyNetEngine: bias / dropout are served by the module path (net.NoisyNet(fused=True), or the "
+        if a.use_bias:
+            raise NotImplementedError("NoisyNetEngine: bias is served by the module path (net.NoisyNet(fused=True), or the "
                                       "unchanged script on the drop-in modules), not the engine")
+        if not 0.0 <= float(a.dropout) < 1.0:
+            raise ValueError("NoisyNetEngine: dropout must lie in [0, 1)")
         if any(getattr(a, k, 0) for k in ("distort_act", "uniform_ind", "uniform_dep", "normal_ind", "normal_dep")):
             raise NotImplementedError("NoisyNetEngine: alternative noise models are served by the module path")
         for li, mod in enumerate((model.conv1, model.conv2, model.linear1, model.linear2)):
@@ -88,6 +93,12 @@ class NoisyNetEngine:
         self.gx3 = f32(B, C2, P2, P2); self.gyp2 = bf16(B, H2, H2, c8(C2))
         self.gx2 = f32(B, C1, P1, P1); self.gyp1 = bf16(B, H1, H1, c8(C1))     # re-laid out below if conv1's wgrad is in-place
         self.loss = f32(1)
+        # dropout (noisynet.py:456-457, :512-513, :565-566): one keep mask per active site, in the BN input's layout.  The
+        # rate is --dropout at every site; --dropout_conv only switches the conv site on (net.NoisyNet does the same)
+        self.drop_p = float(a.dropout)
+        on = (self.drop_p > 0 and a.dropout_conv > 0, self.drop_p > 0, self.drop_p > 0)
+        u8 = lambda *s: torch.zeros(*s, dtype=torch.uint8, device=dev)
+        self.keep = [u8(B, C1, P1, P1) if on[0] else None, u8(B, C2, P2, P2) if on[1] else None, u8(B, FC) if on[2] else None]
         self.scratch = torch.zeros(int(self.lib.nn_stage_scratch_bytes(max(C1, C2, FC))) + 64, dtype=torch.uint8, device=dev)
         # weight packs of the step: forward (4 layers) + dgrad (fc2, fc1 as a linear, conv2), one launch
         modes = [NOISE_MERGED if a.merged_dac else NOISE_EXTERNAL, NOISE_EXTERNAL,
@@ -158,7 +169,8 @@ class NoisyNetEngine:
         for p in model.parameters():
             if p.grad is None:
                 p.grad = torch.zeros_like(p)
-        self.inject = None          # parity hook: dict(u=[...], z=[...]) consumed in the reference's draw order
+        self._keep_inj = []         # injected keep masks of the step being enqueued
+        self.inject = None          # parity hook: dict(u=[...], z=[...], keep=[...]) consumed in the reference's draw order
         self.steps_done = 0         # training steps since the last sync_bn_counters()
         self.logits = f32(B, 10)    # eval_forward output
 
@@ -237,7 +249,7 @@ class NoisyNetEngine:
         return torch.cuda.current_stream(self.di).cuda_stream
 
     def _take(self, kind):
-        if self.inject is None or not self.inject[kind]:
+        if self.inject is None or not self.inject.get(kind):
             return None
         return self.inject[kind].pop(0)
 
@@ -305,7 +317,7 @@ class NoisyNetEngine:
         _lib.check(self.lib.nn_noisy_conv_dgrad(C.byref(a), self.di, self._st()), "nn_noisy_conv_dgrad")
 
     def _stage_fwd(self, x_in, C_, H, pool, pooled, amax, bn, key, q_bits, q_hi, xp, xmax, u=None, act_max=None, eval_mode=False,
-                   stats_ready=False):
+                   stats_ready=False, site=None):
         a = StageArgs()
         a.eval_mode = 1 if eval_mode else 0
         a.stats_ready = 1 if stats_ready else 0
@@ -324,9 +336,16 @@ class NoisyNetEngine:
         a.xp, a.Cp = _p(xp), xp.shape[-1]
         a.act, a.xmax_out = None, _p(xmax)
         a.scratch = _p(self.scratch)
+        keep = self.keep[site] if site is not None else None
+        if keep is not None and not eval_mode:             # dropout is the identity in eval
+            a.drop_p, a.keep = self.drop_p, _p(keep)
+            ki = self._take("keep")
+            self._keep_inj.append(ki)                      # alive until the launch has run
+            a.keep_inject = _p(ki)
+            a.drop_rng = Rng(0, 0, None) if ki is not None else self._rng()     # drawn only when p > 0
         _lib.check(self.lib.nn_stage_fwd(C.byref(a), self.di, self._st()), "nn_stage_fwd")
 
-    def _stage_bwd(self, g, x, amax, C_, H, pool, bn, key, q_bits, q_hi, gyp, planes_grid=None, act_max=None):
+    def _stage_bwd(self, g, x, amax, C_, H, pool, bn, key, q_bits, q_hi, gyp, planes_grid=None, act_max=None, site=None):
         a = StageBwdArgs()
         a.g, a.x, a.argmax = _p(g), _p(x), _p(amax)
         a.B, a.C, a.H, a.W, a.pool = self.B, C_, H, H, pool
@@ -338,6 +357,9 @@ class NoisyNetEngine:
         if planes_grid is not None:
             a.gy_layout, a.virt_H, a.virt_W = PACK_SHIFT, planes_grid[0], planes_grid[1]
         a.scratch = _p(self.scratch)
+        keep = self.keep[site] if site is not None else None
+        if keep is not None:
+            a.drop_p, a.keep = self.drop_p, _p(keep)
         _lib.check(self.lib.nn_stage_bwd(C.byref(a), self.di, self._st()), "nn_stage_bwd")
 
     def _qhi(self, qm):
@@ -371,6 +393,7 @@ class NoisyNetEngine:
         self.w_cs = [(_f32(max(2.0 / (2.0 ** b - 1.0), 1e-6)) / 2.0 if b > 0 else 0.0) for b in self.q_w]
         # ---- weights: quantize (stochastic rounding) + pack for forward and dgrad, all layers, ONE launch
         self._uw_keep = []
+        self._keep_inj = []
         for li in range(4):
             uw = self._take("uw")
             self._uw_keep.append(uw)             # keep injected tensors alive until the launch below has run
@@ -411,22 +434,25 @@ class NoisyNetEngine:
             self._fwd_gemm(0, self.xp1, s1, None, self.noise_modes[0], self._absmax(0, W[0]), self._take("z"),
                            pooled=self.pool1, argmax=self.amax1, bn=m.bn1, key="bn1", zero=self.xmax2)
             self._stage_fwd(self.pool1, C1, P1, 0, None, None, m.bn1, "bn1", a.q_a2, qh2, self.xp2, self.xmax2, self._take("u"), act_max=am1,
-                            stats_ready=True)
+                            stats_ready=True, site=0)
         else:
             self._fwd_gemm(0, self.xp1, s1, self.y1n, self.noise_modes[0], self._absmax(0, W[0]), self._take("z"))
-            self._stage_fwd(self.y1n, C1, H1, 1, self.pool1, self.amax1, m.bn1, "bn1", a.q_a2, qh2, self.xp2, self.xmax2, self._take("u"), act_max=am1)
+            self._stage_fwd(self.y1n, C1, H1, 1, self.pool1, self.amax1, m.bn1, "bn1", a.q_a2, qh2, self.xp2, self.xmax2, self._take("u"), act_max=am1,
+                            site=0)
         if self.side is not None:
             torch.cuda.current_stream(di).wait_stream(self.side)
         self._fwd_gemm(1, self.xp2, s2, self.y2n, self.noise_modes[1], self.xmax2, self._take("z"))
-        self._stage_fwd(self.y2n, C2, H2, 1, self.pool2, self.amax2, m.bn2, "bn2", a.q_a3, qh3, self.xp3, None, self._take("u"), act_max=am2)
+        self._stage_fwd(self.y2n, C2, H2, 1, self.pool2, self.amax2, m.bn2, "bn2", a.q_a3, qh3, self.xp3, None, self._take("u"), act_max=am2,
+                        site=1)
         z3 = self._take("z")
         if self.fuse_bn3 and z3 is None:        # (injected draws run the general epilogue, which is not split over K)
             self._fwd_gemm(2, self.xp3, s3, self.l1n, self.noise_modes[2], self._absmax(2, W[2]), None, bn=m.bn3, key="bn3", zero=self.xmax4)
             self._stage_fwd(self.l1n, FC, 1, 0, None, None, m.bn3, "bn3", a.q_a4, qh4, self.xp4, self.xmax4, self._take("u"), act_max=am3,
-                            stats_ready=True)
+                            stats_ready=True, site=2)
         else:
             self._fwd_gemm(2, self.xp3, s3, self.l1n, self.noise_modes[2], self._absmax(2, W[2]), z3)
-            self._stage_fwd(self.l1n, FC, 1, 0, None, None, m.bn3, "bn3", a.q_a4, qh4, self.xp4, self.xmax4, self._take("u"), act_max=am3)
+            self._stage_fwd(self.l1n, FC, 1, 0, None, None, m.bn3, "bn3", a.q_a4, qh4, self.xp4, self.xmax4, self._take("u"), act_max=am3,
+                            site=2)
         bn4 = m.bn4
         if self.fused_tail:
             # fc2 forward + noise, bn4, cross entropy, their backward and the fc2 dgrad: one 8-CTA cluster launch
@@ -455,7 +481,7 @@ class NoisyNetEngine:
             # ---- backward
             self._wgrad(3, self.gyp4, self.xp4, s4, W[3], W[3].grad)
             self._dgrad(self.geom[3], self.gyp4, 3, self.gx4)
-        self._stage_bwd(self.gx4, self.l1n, None, FC, 1, 0, m.bn3, "bn3", a.q_a4, qh4, self.gyp3, act_max=am3)
+        self._stage_bwd(self.gx4, self.l1n, None, FC, 1, 0, m.bn3, "bn3", a.q_a4, qh4, self.gyp3, act_max=am3, site=2)
         self._wgrad(2, self.gyp3, self.xp3, s3, W[2], W[2].grad)
         if self.red is not None:        # fc gradients (85 % of the payload) travel while the conv backward runs
             if self.side is not None:
@@ -464,7 +490,7 @@ class NoisyNetEngine:
             else:
                 self.red.start_early()
         self._dgrad(self.geom_fc1_lin, self.gyp3, 2, self.gx3)
-        self._stage_bwd(self.gx3, self.pool2, self.amax2, C2, H2, 1, m.bn2, "bn2", a.q_a3, qh3, self.gyp2, act_max=am2)
+        self._stage_bwd(self.gx3, self.pool2, self.amax2, C2, H2, 1, m.bn2, "bn2", a.q_a3, qh3, self.gyp2, act_max=am2, site=1)
         self._wgrad(1, self.gyp2, self.xp2, s2, W[1], W[1].grad)
         if self.red is not None:        # second early bucket: conv2's weight gradient
             if self.side is not None:
@@ -484,7 +510,7 @@ class NoisyNetEngine:
                 self.opt.step_part([W[3], W[2], W[1]], advance=False)
         self._dgrad(self.geom[1], self.gyp2, 1, self.gx2)
         self._stage_bwd(self.gx2, self.pool1, self.amax1, C1, H1, 1, m.bn1, "bn1", a.q_a2, qh2, self.gyp1,
-                        planes_grid=(32, 32) if self.gy1_layout else None, act_max=am1)
+                        planes_grid=(32, 32) if self.gy1_layout else None, act_max=am1, site=0)
         self._wgrad(0, self.gyp1, self.xp1, s1, W[0], W[0].grad, self.gy1_layout)
         # ---- exchange + update
         if self.side is not None:
