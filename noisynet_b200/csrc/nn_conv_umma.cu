@@ -1796,16 +1796,47 @@ static int nn_num_sms_cached() {
     return nn_num_sms(dev);
 }
 
+// per-CTA phase stamps of the forward launches (tools/cta_timeline.py): debug builds with NN_UMMA_DEBUG set
+static bool umma_cta_dbg() {
+#ifdef NN_KDEBUG
+    static const bool on = getenv("NN_UMMA_DEBUG") != nullptr;
+    return on;
+#else
+    return false;
+#endif
+}
+
+// the epilogue k_conv_umma is instantiated with (see k_conv_umma)
+static int umma_epi(const UmmaP& p) {
+    const bool extras = p.bias || p.mask_x || p.z_inject || p.z_export || p.sigma_export || p.stats;
+    if (!extras && p.main_col >= 0 && p.noise_mode != NN_NOISE_NONE && p.y_noisy) return 1;
+    if (!extras && p.main_col >= 0 && p.noise_mode == NN_NOISE_NONE && p.y) return 2;
+    return 0;
+}
+
+// split-K for skinny linear layers (few m-tiles x n-tiles, long K: fc1 forward at batch 512 is 52 CTAs walking 47
+// k-blocks each -- a latency chain on a third of the SMs): the k-blocks are dealt to this many CTAs per tile, which dump
+// raw accumulators, and k_splitk_epilogue sums them and applies the noise epilogue.  1 = not split (also when the
+// split-K workspace, ws_bytes, cannot hold the partial sums)
+static int umma_splits(const UmmaP& p, const Plan& pl, size_t ws_bytes) {
+    const int epi = umma_epi(p);
+    const int m_tiles = (p.M + UM_BLOCK_M - 1) / UM_BLOCK_M;
+    if ((epi != 1 && epi != 2) || p.OH * p.OW != 1 || umma_cta_dbg() || m_tiles * pl.n_tiles * 2 > nn_num_sms_cached() ||
+        pl.num_kb < 8 || ws_bytes == 0)
+        return 1;
+    int splits = 4;
+    while (splits > 1 && pl.num_kb / splits < 4) --splits;
+    const size_t need = (size_t)splits * pl.n_tiles * pl.n_mma * m_tiles * UM_BLOCK_M * sizeof(float);
+    return need > ws_bytes ? 1 : splits;
+}
+
 static int launch_umma(const UmmaP& p, const Plan& pl, cudaStream_t st, void* splitk_ws = nullptr, size_t splitk_ws_bytes = 0) {
     NN_ONCE_PER_DEVICE({
         NN_CUDA_OK(cudaFuncSetAttribute(k_conv_umma<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         NN_CUDA_OK(cudaFuncSetAttribute(k_conv_umma<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
         NN_CUDA_OK(cudaFuncSetAttribute(k_conv_umma<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     });
-    const bool extras = p.bias || p.mask_x || p.z_inject || p.z_export || p.sigma_export || p.stats;
-    int epi = 0;
-    if (!extras && p.main_col >= 0 && p.noise_mode != NN_NOISE_NONE && p.y_noisy) epi = 1;
-    else if (!extras && p.main_col >= 0 && p.noise_mode == NN_NOISE_NONE && p.y) epi = 2;
+    const int epi = umma_epi(p);
     UmmaP pd = p;
     // incremental tap tracking saves the producers' divisions on the plain (dgrad) variant; the noisy forward keeps the
     // direct computation
@@ -1813,7 +1844,7 @@ static int launch_umma(const UmmaP& p, const Plan& pl, cudaStream_t st, void* sp
     pd.rows_tile = UM_BLOCK_M;
     dim3 grid((p.M + pd.rows_tile - 1) / pd.rows_tile, pl.n_tiles);
 #ifdef NN_KDEBUG
-    static const bool want_dbg = getenv("NN_UMMA_DEBUG") != nullptr;      // per-CTA phase stamps (tools/cta_timeline.py)
+    const bool want_dbg = umma_cta_dbg();
     if (want_dbg) {
         const size_t ctas = (size_t)grid.x * grid.y;
         if (ctas > g_dbg_ctas) {
@@ -1825,19 +1856,8 @@ static int launch_umma(const UmmaP& p, const Plan& pl, cudaStream_t st, void* sp
         pd.dbg = g_dbg_buf;
         g_dbg_last = ctas;
     }
-#else
-    const bool want_dbg = false;
 #endif
-    // split-K for skinny linear layers (few m-tiles x n-tiles, long K: fc1 forward at batch 512 is 52 CTAs walking 47
-    // k-blocks each -- a latency chain on a third of the SMs): the k-blocks are dealt to gridDim.z CTAs that dump raw
-    // accumulators, and k_splitk_epilogue sums them and applies the noise epilogue
-    int splits = 1;
-    if ((epi == 1 || epi == 2) && p.OH * p.OW == 1 && !want_dbg && (int)(grid.x * grid.y) * 2 <= nn_num_sms_cached() && pl.num_kb >= 8 && splitk_ws) {
-        splits = 4;
-        while (splits > 1 && pl.num_kb / splits < 4) --splits;
-        const size_t need = (size_t)splits * pl.n_tiles * pl.n_mma * grid.x * UM_BLOCK_M * sizeof(float);
-        if (need > splitk_ws_bytes) splits = 1;
-    }
+    const int splits = umma_splits(p, pl, splitk_ws ? splitk_ws_bytes : 0);
     if (splits > 1) {
         grid.z = splits;
         pd.partial = (float*)splitk_ws;
@@ -1883,8 +1903,7 @@ static int launch_umma(const UmmaP& p, const Plan& pl, cudaStream_t st, void* sp
         e.main_col = pl.main_col; e.sig_col = pl.sig_col; e.m_pad = pd.m_pad; e.M = p.M; e.Cout = p.Cout;
         e.y_scale = p.y_scale; e.s_scale = p.s_scale; e.current = p.current; e.scale_dev = p.scale_dev; e.rng = p.rng;
         e.y = p.y; e.y_noisy = p.y_noisy; e.noisy = epi == 1;
-        if (p.bn_fin.mean) {
-            if (p.M % 256) return nn_fail("nn_noisy_conv_fwd: bn_mean on a linear layer needs a batch that is a multiple of 256%s", "");
+        if (p.bn_fin.mean) {        // (nn_umma_conv_fwd checked M % 256 == 0)
             e.stat_partial = (double*)p.bn_scratch;
             e.stat_counters = (unsigned*)(e.stat_partial + (size_t)p.Cout * 16 * 2);
             e.fin = p.bn_fin; e.fin.count = (double)p.M; e.zero_out = p.zero_out;
@@ -1892,8 +1911,6 @@ static int launch_umma(const UmmaP& p, const Plan& pl, cudaStream_t st, void* sp
         const int total = p.M * ((p.Cout + 3) / 4);
         k_splitk_epilogue<<<(total + 255) / 256, 256, 0, st>>>(e);
         NN_LAUNCH_OK();
-    } else if (p.bn_fin.mean) {
-        return nn_fail("nn_noisy_conv_fwd: bn_mean on a linear layer is served by the split-K epilogue only%s (see nn_conv_linear_bn_fusable)", "");
     }
     return 0;
 }
@@ -2240,34 +2257,9 @@ int nn_umma_conv_fwd(const nn_conv_fwd_args* a, int device, cudaStream_t st) {
     if (!a->workspace || (size_t)a->workspace_bytes < need)
         return nn_fail("nn_noisy_conv_fwd: workspace too small%s (need %lld bytes)", "", (long long)need);
     uint8_t* ws = (uint8_t*)align_up((size_t)a->workspace, 1024);
-    __nv_bfloat16* xp = (__nv_bfloat16*)ws;
-    __nv_bfloat16* wp = (__nv_bfloat16*)(ws + align_up(pl.xp_bytes, 1024));
+    __nv_bfloat16* xp = a->x_packed ? (__nv_bfloat16*)a->x_packed : (__nv_bfloat16*)ws;
+    __nv_bfloat16* wp = a->w_packed ? (__nv_bfloat16*)a->w_packed : (__nv_bfloat16*)(ws + align_up(pl.xp_bytes, 1024));
     int* err = nn_umma_err_flag(device);
-
-    if (a->x_packed) {
-        xp = (__nv_bfloat16*)a->x_packed;
-    } else {   // activations -> NHWC bf16 (integer codes when a_code_scale > 0)
-        const int64_t total = (int64_t)g.B * g.H * g.W * (pl.Cp / 8);
-        int grid = (int)((total + 255) / 256);
-        if (grid > 16 * nn_num_sms(device)) grid = 16 * nn_num_sms(device);
-        k_pack_act<<<grid, 256, 0, st>>>(a->x, xp, g.B, g.Cin, g.H * g.W, pl.Cp, a->a_code_scale);
-        NN_LAUNCH_OK();
-    }
-    if (a->w_packed) {
-        wp = (__nv_bfloat16*)a->w_packed;
-    } else {
-        PackWP pw;
-        memset(&pw, 0, sizeof(pw));
-        pw.w_eff = a->w_eff; pw.w_raw = a->w_raw; pw.wp = wp;
-        pw.Cout = g.Cout; pw.Cin = g.Cin; pw.KHW = g.KH * g.KW; pw.Cp = pl.Cp; pw.n_t = pl.n_t; pw.n_mma = pl.n_mma;
-        pw.num_kb = pl.num_kb; pw.n_tiles = pl.n_tiles; pw.main_col = pl.main_col; pw.sig_col = pl.sig_col;
-        pw.wsum_col = pl.wsum_col; pw.noise_mode = a->noise_mode; pw.mode = 0; pw.w_code_scale = a->w_code_scale;
-        const int64_t total = (int64_t)pl.n_tiles * pl.num_kb * pl.n_mma * 8;
-        int grid = (int)((total + 255) / 256);
-        if (grid > 8 * nn_num_sms(device)) grid = 8 * nn_num_sms(device);
-        k_pack_w<<<grid, 256, 0, st>>>(pw);
-        NN_LAUNCH_OK();
-    }
     UmmaP p;
     memset(&p, 0, sizeof(p));
     p.B = g.B; p.H = g.H; p.W = g.W; p.Cp = pl.Cp; p.KH = g.KH; p.KW = g.KW; p.stride = g.stride; p.pad = g.pad;
@@ -2282,20 +2274,47 @@ int nn_umma_conv_fwd(const nn_conv_fwd_args* a, int device, cudaStream_t st) {
     p.noise_mode = a->noise_mode; p.current = a->current; p.scale_dev = a->scale_dev; p.z_inject = a->z_inject;
     p.z_export = a->z_export; p.sigma_export = a->sigma_export; p.stats = a->stats; p.rng = a->rng;
     p.mask_x = nullptr; p.err_flag = err;
+    // what is left of the workspace after the operand packs serves the split-K partial sums
+    uint8_t* rest = ws + align_up(pl.xp_bytes, 1024) + align_up(pl.wp_bytes, 1024);
+    uint8_t* ws_end = (uint8_t*)a->workspace + a->workspace_bytes;
+    void* splitk_ws = rest < ws_end ? rest : nullptr;
+    const size_t splitk_bytes = rest < ws_end ? (size_t)(ws_end - rest) : 0;
     if (a->bn_mean && !a->pooled_out) {       // BatchNorm1d statistics of a linear layer's output from the split-K epilogue
+        // (every refusal comes before the first launch: a refused call writes nothing)
         if (!a->bn_invstd || !a->bn_scratch) return nn_fail("nn_noisy_conv_fwd: bn_mean needs bn_invstd and bn_scratch%s", "");
         if (a->bn_eval_mode && (!a->bn_running_mean || !a->bn_running_var))
             return nn_fail("nn_noisy_conv_fwd: bn_eval_mode needs the running statistics%s", "");
         if (g.Cout > 0 && ((g.B * OH * OW) >> 8) > 16) return nn_fail("nn_noisy_conv_fwd: bn_mean on a linear layer serves batches up to 4096%s", "");
+        if (p.M % 256) return nn_fail("nn_noisy_conv_fwd: bn_mean on a linear layer needs a batch that is a multiple of 256%s", "");
+        if (umma_splits(p, pl, splitk_bytes) == 1)
+            return nn_fail("nn_noisy_conv_fwd: bn_mean on a linear layer is served by the split-K epilogue only%s (see nn_conv_linear_bn_fusable)", "");
         p.bn_fin.mean = a->bn_mean; p.bn_fin.invstd = a->bn_invstd; p.bn_fin.running_mean = a->bn_running_mean;
         p.bn_fin.running_var = a->bn_running_var; p.bn_fin.eps = a->bn_eps; p.bn_fin.momentum = a->bn_momentum;
         p.bn_fin.eval_mode = a->bn_eval_mode; p.bn_fin.xmax_out = nullptr;
         p.bn_scratch = a->bn_scratch; p.zero_out = a->zero_out;
     }
-    // what is left of the workspace after the operand packs serves the split-K partial sums
-    uint8_t* rest = ws + align_up(pl.xp_bytes, 1024) + align_up(pl.wp_bytes, 1024);
-    uint8_t* ws_end = (uint8_t*)a->workspace + a->workspace_bytes;
-    return launch_umma(p, pl, st, rest < ws_end ? rest : nullptr, rest < ws_end ? (size_t)(ws_end - rest) : 0);
+
+    if (!a->x_packed) {   // activations -> NHWC bf16 (integer codes when a_code_scale > 0)
+        const int64_t total = (int64_t)g.B * g.H * g.W * (pl.Cp / 8);
+        int grid = (int)((total + 255) / 256);
+        if (grid > 16 * nn_num_sms(device)) grid = 16 * nn_num_sms(device);
+        k_pack_act<<<grid, 256, 0, st>>>(a->x, xp, g.B, g.Cin, g.H * g.W, pl.Cp, a->a_code_scale);
+        NN_LAUNCH_OK();
+    }
+    if (!a->w_packed) {
+        PackWP pw;
+        memset(&pw, 0, sizeof(pw));
+        pw.w_eff = a->w_eff; pw.w_raw = a->w_raw; pw.wp = wp;
+        pw.Cout = g.Cout; pw.Cin = g.Cin; pw.KHW = g.KH * g.KW; pw.Cp = pl.Cp; pw.n_t = pl.n_t; pw.n_mma = pl.n_mma;
+        pw.num_kb = pl.num_kb; pw.n_tiles = pl.n_tiles; pw.main_col = pl.main_col; pw.sig_col = pl.sig_col;
+        pw.wsum_col = pl.wsum_col; pw.noise_mode = a->noise_mode; pw.mode = 0; pw.w_code_scale = a->w_code_scale;
+        const int64_t total = (int64_t)pl.n_tiles * pl.num_kb * pl.n_mma * 8;
+        int grid = (int)((total + 255) / 256);
+        if (grid > 8 * nn_num_sms(device)) grid = 8 * nn_num_sms(device);
+        k_pack_w<<<grid, 256, 0, st>>>(pw);
+        NN_LAUNCH_OK();
+    }
+    return launch_umma(p, pl, st, splitk_ws, splitk_bytes);
 }
 
 static Plan plan_for_job(const nn_wprep_job& jb) {
