@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define NN_ABI_VERSION 16
+#define NN_ABI_VERSION 17
 
 /* ---- common ---------------------------------------------------------------------- */
 
@@ -171,7 +171,10 @@ typedef struct nn_conv_fwd_args {
     int64_t workspace_bytes;
     const void* x_packed;    /* optional (tensor-core precisions): the input already packed as NHWC bf16
                                 [B,H,W,ceil8(Cin)] (codes if a_code_scale > 0), e.g. by nn_stage_fwd;
-                                `x` is then ignored and the pack kernel is skipped                    */
+                                `x` is then ignored and the pack kernel is skipped.  A launch on
+                                NN_PACK_SHIFT weights (w_packed_layout, or nn_conv_pack_layout when
+                                the weights are not packed) takes the ROW-PLANE image instead
+                                (nn_conv_shift_planes_bytes, nn_input_quant_pack_rows)                */
     const void* w_packed;    /* optional: weights already packed by nn_prepare_weights (mode 0, same
                                 noise_mode / stats choice); w_eff may then be NULL, w_code_scale must be
                                 the quantizer's s/2                                                   */
@@ -199,10 +202,11 @@ int64_t nn_conv_bn_scratch_bytes(int Cout);
 int nn_conv_linear_bn_fusable(const nn_conv_geom* g, int32_t noise_mode, int32_t precision, int device);
 
 /* Packed-weight layouts.  NN_PACK_TILED: 128B-swizzled [n-tile][k-block] shared-memory images (every geometry).
- * NN_PACK_SHIFT: [tap][row][8] image of the persistent shift-GEMM forward kernel, served for stride-1 unpadded
- * layers with Cin <= 8 (the first layer, noisynet.py:344): ask nn_conv_pack_layout which one the forward of a
- * geometry prefers; nn_noisy_conv_fwd rejects a layout it cannot serve (bias / stats / export requests need
- * NN_PACK_TILED). */
+ * NN_PACK_SHIFT: [kh][plane][row][8] image of the persistent shift-GEMM forward kernel (k = kw * Cin + c of kernel
+ * row kh, 8 per plane, P = 2 ceil(KW Cin / 16) planes; nn_prepare_weights packs square kernels, KH = KW =
+ * sqrt(KHW)), served for stride-1 unpadded layers with Cin <= 8 (the first layer, noisynet.py:344): ask
+ * nn_conv_pack_layout which one the forward of a geometry prefers; nn_noisy_conv_fwd rejects a layout it cannot
+ * serve (bias / stats / export requests need NN_PACK_TILED). */
 #define NN_PACK_TILED 0
 #define NN_PACK_SHIFT 1
 /* NN_PACK_TMA: [n-tile][tap][stage][CTA rank] image of the persistent CTA-pair kernel whose activations arrive by
@@ -210,6 +214,10 @@ int nn_conv_linear_bn_fusable(const nn_conv_geom* g, int32_t noise_mode, int32_t
  * more than 8 input channels, square kernels) on the lean path (no bias / statistics / exports / clean-output copy). */
 #define NN_PACK_TMA 2
 int nn_conv_pack_layout(const nn_conv_geom* g, int32_t noise_mode, int32_t precision);
+/* Bytes of the row-plane input image of an NN_PACK_SHIFT forward: P = 2 ceil(KW Cin / 16) planes [plane][B][H][W][8]
+ * bf16; element j of plane q at pixel (b, h, w) is x[b, c, h, w + kw] for kw * Cin + c = 8 q + j, zero where
+ * w + kw >= W or 8 q + j >= KW * Cin.  0 for Cin outside 1..8. */
+int64_t nn_conv_shift_planes_bytes(const nn_conv_geom* g);
 /* Layout the dgrad of a geometry prefers for its (transposed, tap-flipped) weight image: NN_PACK_TMA or NN_PACK_TILED. */
 int nn_conv_dgrad_pack_layout(const nn_conv_geom* g, int32_t precision);
 /* Test hook: enable = 0/1 switches the TMA-im2col path off/on (< 0: query); returns the previous setting. */
@@ -370,6 +378,12 @@ int nn_stage_bwd(const nn_stage_bwd_args* a, int device, void* stream);
 /* Input quantizer (quantize1, noisynet.py:344, :390-393) + NHWC bf16 code pack of the network input. */
 int nn_input_quant_pack(const float* x, void* xp, float* act, int B, int C, int HW, int Cp, int q_bits,
                         double q_hi, float stochastic, const float* u_inject, nn_rng rng, int device, void* stream);
+/* The same codes (same arithmetic and Philox counters: bit-identical) as the row-plane image `planes` of a KW-wide shift
+ * forward (nn_conv_shift_planes_bytes of the geometry, C <= 8) and, if xp != NULL, the NHWC image [B,H,W,8] of
+ * nn_input_quant_pack with Cp = 8, from one pass over x [B,C,H,W].  x = NULL: the planes are made from the NHWC code
+ * image xp instead (e.g. written by nn_input_gather_quant_pack). */
+int nn_input_quant_pack_rows(const float* x, void* xp, void* planes, int B, int C, int H, int W, int KW, int q_bits,
+                             double q_hi, float stochastic, const float* u_inject, nn_rng rng, int device, void* stream);
 
 /* Data path (section 8f.4): batch assembly of noisynet.py:1232-1269 on the device -- gather B images BY INDEX (idx [B]
  * int64 on the device, NULL = the first B) from the resident, zero-padded dataset [N,C,Hp,Wp] fp32 (utils.py:165-167), crop

@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("NN_LIB_PATH") or os.path.join(_HERE, "lib", "libnoisynet_b200.so")   # NN_LIB_PATH: instrumented debug builds
-ABI_VERSION = 16
+ABI_VERSION = 17
 
 NOISE_NONE, NOISE_MERGED, NOISE_EXTERNAL = 0, 1, 2
 PREC_FP32, PREC_TF32, PREC_BF16 = 0, 1, 2
@@ -142,6 +142,8 @@ SIGNATURES = {
     "nn_stage_bwd": (C.c_int, [C.POINTER(StageBwdArgs), C.c_int, C.c_void_p]),
     "nn_input_quant_pack": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                       C.c_double, C.c_float, C.c_void_p, Rng, C.c_int, C.c_void_p]),
+    "nn_input_quant_pack_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                           C.c_int, C.c_double, C.c_float, C.c_void_p, Rng, C.c_int, C.c_void_p]),
     "nn_input_gather_quant_pack": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                              C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double,
                                              C.c_float, C.c_void_p, Rng, C.c_int, C.c_void_p]),
@@ -173,6 +175,7 @@ SIGNATURES = {
     "nn_classifier_tail": (C.c_int, [C.POINTER(TailArgs), C.c_int, C.c_void_p]),
     "nn_conv_wgrad_pack_layout": (C.c_int, [C.POINTER(ConvGeom), C.c_int32, C.c_int]),
     "nn_conv_gy_planes_bytes": (C.c_int64, [C.POINTER(ConvGeom)]),
+    "nn_conv_shift_planes_bytes": (C.c_int64, [C.POINTER(ConvGeom)]),
     "nn_noisy_conv_fwd": (C.c_int, [C.POINTER(ConvFwdArgs), C.c_int, C.c_void_p]),
     "nn_noisy_conv_dgrad": (C.c_int, [C.POINTER(ConvDgradArgs), C.c_int, C.c_void_p]),
     "nn_conv_wgrad_workspace_bytes": (C.c_int64, [C.POINTER(ConvGeom), C.c_int32, C.c_int]),

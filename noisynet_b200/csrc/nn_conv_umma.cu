@@ -483,22 +483,24 @@ k_splitk_epilogue(const SplitEpiP p) {
 }
 
 // ================================================================== shift-GEMM forward (narrow-input layers)
-// For a stride-1, unpadded conv whose input has <= 8 channels (the first layer: 3 -> Cp = 8, ONE 16-byte
-// chunk per pixel), the im2col rows of tap (kh, kw) are the packed pixels themselves, shifted by kh*W + kw:
-// with the SWIZZLE_NONE ("interleave") K-major descriptor a core matrix is 8 rows x 16 B = 8 CONSECUTIVE
-// PIXELS of the NHWC pack, so the A operand of every tap is the same shared-memory tile read through a
-// shifted start address -- nothing is gathered.  An m-tile is 128 consecutive positions of the INPUT pixel
-// grid ("virtual" outputs: positions with ow >= OW or oh >= OH are computed and dropped, 12.5 % for 32 -> 28),
-// staged by ONE cp.async.bulk of (128 + (KH-1) W + KW-1) pixels = 4 KB instead of 64 KB of gathered im2col.
-// The whole weight image (taps x rows, 60 KB) stays resident in shared memory, so the CTA is persistent:
+// For a stride-1, unpadded conv whose input has <= 8 channels (the first layer: 3), the K dimension of kernel row kh is its
+// KW horizontal taps x Cin channels, k = kw * Cin + c (conv1: 15 of 16).  The input arrives as a ROW-PLANE image
+// (nn_conv_shift_planes_bytes): P = 2 ceil(KW Cin / 16) planes [plane][B][H][W][8], element j of plane q at pixel (b, h, w)
+// being x[b, c, h, w + kw] for kw * Cin + c = 8 q + j (zero past the right edge and past KW Cin).  With the SWIZZLE_NONE
+// ("interleave") K-major descriptor a core matrix is 8 rows x 16 B = 8 CONSECUTIVE PIXELS of a plane, so the im2col rows
+// of kernel row kh are the plane pixels themselves, shifted by kh*W: one K = 16 wgmma per (kernel row, plane pair), its
+// two 8-wide K chunks one plane apart (LBO) -- nothing is gathered.  An m-tile is 128 consecutive positions of the INPUT
+// pixel grid ("virtual" outputs: positions with ow >= OW or oh >= OH are computed and dropped, 12.5 % for 32 -> 28),
+// staged by P cp.async.bulk copies of (128 + (KH-1) W) pixels each.  The whole weight image ([kh][plane][row][8],
+// 23 KB for conv1) stays resident in shared memory, so the CTA is persistent:
 //   warps 0 .. SH_EPI_WARPS - 1 : epilogue (scale, Philox/Box-Muller noise -> NCHW stores) from a shared-memory
 //              accumulator tile; warps with (warp & 3) < 2 read its rows 0-63 (half 0), the others rows 64-127 (half 1)
-//   next 8 warps : two MMA warpgroups, one per 64-row half of the tile.  Each issues one K = 16 wgmma per PAIR of taps
-//              (LBO = pixel distance of the two taps) over the accumulator width, and stores its half into the tile as soon
-//              as that half's epilogue warps have released it -- so it runs up to one tile ahead of them.  The first warp of
-//              warpgroup 0 also issues the bulk copies (weights once, then the A ring, which runs ahead of the tiles).
+//   next 8 warps : two MMA warpgroups, one per 64-row half of the tile.  Each issues KH P / 2 wgmmas (conv1: 5) per column
+//              pass over the accumulator width, and stores its half into the tile as soon as that half's epilogue warps
+//              have released it -- so it runs up to one tile ahead of them.  The first warp of warpgroup 0 also issues
+//              the bulk copies (weights once, then the A ring, which runs ahead of the tiles).
 // 24 warps are 6 per SM sub-partition: a cap of 80 registers per thread, which both roles fit without spilling.
-constexpr int SH_MAX_PAIRS = 64;
+constexpr int SH_MAX_STEPS = 64;                    // K = 16 steps of a chain (kernel rows x plane pairs)
 constexpr int SH_STAGES = 2;
 constexpr int SH_MAX_N = 256;                       // accumulator columns
 constexpr int SH_MAX_N1 = 80;                       // widest chain of one column pass (40 accumulators) under the 80-register cap
@@ -506,10 +508,11 @@ constexpr int SH_POOL_IT = 5;                       // pooled launches: 4-channe
 
 struct ShiftP {
     int H, W, OH, OW, KH, KW, Cout;
-    int n_mma, main_col, sig_col, n_pairs;
-    int a_pixels, a_stage, b_bytes, n_tiles;        // pixels / bytes per A stage, weight image bytes, m-tiles
+    int n_mma, main_col, sig_col, n_steps, n_planes;
+    int a_pixels, a_plane, a_stage, b_bytes, n_tiles;   // pixels / bytes per plane of an A stage, bytes per A stage, weight image bytes, m-tiles
+    int acc_bufs;                                       // accumulator tiles (1 or 2): live tile i of a CTA uses tile i % acc_bufs
     long long total_pixels;
-    const __nv_bfloat16 *xp, *wp;
+    const __nv_bfloat16 *xp, *wp;   // xp: the row-plane image, planes total_pixels apart
     float y_scale, s_scale;
     float *y, *y_noisy;
     float* pooled;            // optional: fused MaxPool2d(2,2) of the (noisy) output [B,Cout,OH/2,OW/2]; then y / y_noisy are not written
@@ -560,30 +563,31 @@ __device__ __forceinline__ bool shift_tile_live(const ShiftP& p, int t) {
     return (int)((v0 - b0 * hw) / (unsigned)p.W) < p.OH;
 }
 
-// Tap pairs j0 .. j0 + L - 1 of a half's chain: one m64nNk16 wgmma each, committed as one group.  A: the stage's half at
-// 16-byte unit a16, shifted per pair (tap_tab: shift | lbo << 16); B: the pair's weight rows, b_pair units apart.
+// K = 16 steps j0 .. j0 + L - 1 of a half's chain: one m64nNk16 wgmma each, committed as one group.  A: the stage's half
+// at 16-byte unit a16, shifted per step (tap_tab: shift | lbo << 16); B: the step's weight rows, b_step units apart.
 template <int N, int L>
-__device__ __forceinline__ void shift_chain(float* acc, const uint32_t* tap_tab, uint64_t ad_t, uint32_t a16, uint64_t bd, uint32_t b_pair,
+__device__ __forceinline__ void shift_chain(float* acc, const uint32_t* tap_tab, uint64_t ad_t, uint32_t a16, uint64_t bd, uint32_t b_step,
                                             int j0) {
     wg_fence();
 #pragma unroll
     for (int k = 0; k < L; ++k) {
         const uint32_t e = tap_tab[j0 + k];
         const uint64_t ad = ad_t | (uint64_t)((a16 + (e & 0xFFFFu)) & 0x3FFFu) | ((uint64_t)((e >> 16) & 0x3FFFu) << 16);
-        wgmma_c<N, 0, 0>(acc, ad, bd + (uint64_t)(j0 + k) * b_pair, j0 + k != 0);
+        wgmma_c<N, 0, 0>(acc, ad, bd + (uint64_t)(j0 + k) * b_step, j0 + k != 0);
     }
     wg_commit();
 }
-// the whole chain of a half (n_pairs tap pairs, in blocks of up to 4), drained
+// the whole chain of a half (n_steps K = 16 steps, in blocks of up to 5: a 5 x 5 kernel on 2 planes is one block), drained
 template <int N>
-__device__ __forceinline__ void shift_half_mma(float* acc, const uint32_t* tap_tab, uint64_t ad_t, uint32_t a16, uint64_t bd, uint32_t b_pair,
-                                               int n_pairs) {
-    for (int j0 = 0; j0 < n_pairs; j0 += 4) {
-        switch (min(4, n_pairs - j0)) {
-            case 4: shift_chain<N, 4>(acc, tap_tab, ad_t, a16, bd, b_pair, j0); break;
-            case 3: shift_chain<N, 3>(acc, tap_tab, ad_t, a16, bd, b_pair, j0); break;
-            case 2: shift_chain<N, 2>(acc, tap_tab, ad_t, a16, bd, b_pair, j0); break;
-            default: shift_chain<N, 1>(acc, tap_tab, ad_t, a16, bd, b_pair, j0); break;
+__device__ __forceinline__ void shift_half_mma(float* acc, const uint32_t* tap_tab, uint64_t ad_t, uint32_t a16, uint64_t bd, uint32_t b_step,
+                                               int n_steps) {
+    for (int j0 = 0; j0 < n_steps; j0 += 5) {
+        switch (min(5, n_steps - j0)) {
+            case 5: shift_chain<N, 5>(acc, tap_tab, ad_t, a16, bd, b_step, j0); break;
+            case 4: shift_chain<N, 4>(acc, tap_tab, ad_t, a16, bd, b_step, j0); break;
+            case 3: shift_chain<N, 3>(acc, tap_tab, ad_t, a16, bd, b_step, j0); break;
+            case 2: shift_chain<N, 2>(acc, tap_tab, ad_t, a16, bd, b_step, j0); break;
+            default: shift_chain<N, 1>(acc, tap_tab, ad_t, a16, bd, b_step, j0); break;
         }
     }
     wg_wait_all();
@@ -610,8 +614,8 @@ __host__ __device__ constexpr int shift_passes(int nc) {
     return np;
 }
 
-// the MMA warpgroup's bulk copy of the next live tile from t_ld on into A stage s (the ring is filled in the order it is
-// consumed); the first warp of the warpgroup (loader) issues it
+// the MMA warpgroup's bulk copies of the next live tile from t_ld on into A stage s, one per plane onto the stage's full
+// barrier (the ring is filled in the order it is consumed); the first warp of the warpgroup (loader) issues them
 __device__ __forceinline__ void shift_load_next(const ShiftP& p, uint32_t a_base, uint32_t a_full, int s, bool loader, int& t_ld) {
     while (t_ld < p.n_tiles && !shift_tile_live(p, t_ld)) t_ld += gridDim.x;
     if (t_ld >= p.n_tiles) return;
@@ -622,8 +626,10 @@ __device__ __forceinline__ void shift_load_next(const ShiftP& p, uint32_t a_base
         if (px > p.a_pixels) px = p.a_pixels;
         const uint32_t bytes = (uint32_t)px * 16u;
         if (elect_one_sync()) {
-            mbar_arrive_expect_tx(a_full + 8 * s, bytes);
-            bulk_g2s(a_base + (uint32_t)s * p.a_stage, p.xp + v0 * 8, bytes, a_full + 8 * s);
+            mbar_arrive_expect_tx(a_full + 8 * s, bytes * (uint32_t)p.n_planes);
+            for (int q = 0; q < p.n_planes; ++q)
+                bulk_g2s(a_base + (uint32_t)s * p.a_stage + (uint32_t)q * p.a_plane, p.xp + ((long long)q * p.total_pixels + v0) * 8, bytes,
+                         a_full + 8 * s);
         }
         __syncwarp();
     }
@@ -631,9 +637,11 @@ __device__ __forceinline__ void shift_load_next(const ShiftP& p, uint32_t a_base
 }
 
 // MMA warpgroup h (0 / 1) of k_conv_shift for an accumulator width of NC columns (n_mma), in column passes of at most
-// SH_MAX_N1: per live tile, the chain over rows 64 h .. 64 h + 63 of the resident operands, then -- once the half's epilogue
-// warps have released it (acc_empty[h]) -- the fragments into those rows of the accumulator tile and an arrival on
-// acc_full[h].  The two warpgroups run side by side, each up to a tile ahead of its half's epilogue warps.  The first warp
+// SH_MAX_N1: per live tile i, the chain over rows 64 h .. 64 h + 63 of the resident operands, then -- once the half's
+// epilogue warps have released it (acc_empty[buf][h], buf = i % acc_bufs) -- the fragments into those rows of
+// accumulator tile buf and an arrival on acc_full[buf][h].  The two warpgroups run side by side, each up to acc_bufs
+// tiles ahead of its half's epilogue warps: with two accumulator tiles the stores of tile i + 1, and the second column
+// pass between them, are no longer on the epilogue's path.  The first warp
 // of warpgroup 0 also issues the bulk copies: the weights once, then the A ring, refilling a stage once both chains that
 // read it have completed (its own, and warpgroup 1's arrival on a_empty).  Returns a nonzero abort code when a barrier
 // wait times out.
@@ -660,12 +668,12 @@ __device__ __forceinline__ uint32_t shift_mma_role(const ShiftP& p, int h, uint3
     }
     if (!mbar_wait(b_full, 0)) return 2;
     const uint64_t bd0 = gmma_desc_none(b_base, (uint32_t)NC, 8u);
-    const uint64_t ad_t = gmma_desc_none(0u, 0u, (uint32_t)p.sbo_units);     // A template: start address and LBO vary per tap pair
-    const uint32_t b_pair = 2u * NC;
+    const uint64_t ad_t = gmma_desc_none(0u, 0u, (uint32_t)p.sbo_units);     // A template: start address and LBO come from tap_tab
+    const uint32_t b_step = 2u * NC;
     int i = 0;
     for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
         if (!shift_tile_live(p, t)) continue;
-        const int s = i & 1;
+        const int s = i & 1, buf = p.acc_bufs > 1 ? (i & 1) : 0;
         const uint32_t ph = ((uint32_t)i >> 1) & 1u;
         if (!mbar_wait(a_full + 8 * s, ph)) return 4;
         if (*abort_g) return 0;
@@ -674,7 +682,7 @@ __device__ __forceinline__ uint32_t shift_mma_role(const ShiftP& p, int h, uint3
 #pragma unroll
         for (int c = 0; c < NP; ++c) {
             float acc[N / 2];
-            shift_half_mma<N>(acc, tap_tab, ad_t, a16h, bd0 + (uint64_t)(c * N), b_pair, p.n_pairs);
+            shift_half_mma<N>(acc, tap_tab, ad_t, a16h, bd0 + (uint64_t)(c * N), b_step, p.n_steps);
             if (c == NP - 1) {          // this warpgroup's chains over stage s have completed
                 if (h == 1) {
                     if (first_warp && elect_one_sync()) mbar_arrive(a_empty + 8 * s);
@@ -684,11 +692,11 @@ __device__ __forceinline__ uint32_t shift_mma_role(const ShiftP& p, int h, uint3
                     shift_load_next(p, a_base, a_full, s, true, t_ld);
                 }
             }
-            if (c == 0 && !mbar_wait(acc_empty + 8 * h, ((uint32_t)i & 1u) ^ 1u)) return 6;
-            shift_acc_store<N>(acc, acc_tile, 64 * h, c * N);
+            if (c == 0 && !mbar_wait(acc_empty + 8 * (2 * buf + h), ((uint32_t)(i / p.acc_bufs) & 1u) ^ 1u)) return 6;
+            shift_acc_store<N>(acc, acc_tile, 128 * buf + 64 * h, c * N);
         }
         __syncwarp();
-        if (elect_one_sync()) mbar_arrive(acc_full + 8 * h);
+        if (elect_one_sync()) mbar_arrive(acc_full + 8 * (2 * buf + h));
         __syncwarp();
         if (first_warp && (threadIdx.x & 31) == 0) shift_dbg(p, i, 1 + h);
         ++i;
@@ -711,35 +719,33 @@ k_conv_shift(const ShiftP p) {
     const uint32_t bar_base = a_base + (uint32_t)SH_STAGES * (uint32_t)p.a_stage;
     const uint32_t a_full = bar_base, a_empty = bar_base + 8u * SH_STAGES;
     const uint32_t b_full = bar_base + 16u * SH_STAGES;
-    const uint32_t acc_full = b_full + 8u, acc_empty = acc_full + 16u;          // per accumulator half
-    const uint32_t abort_slot = acc_empty + 16u, tab_slot = abort_slot + 4u;
-    const uint32_t pool_slot = (tab_slot + 4u * SH_MAX_PAIRS + 15u) & ~15u;      // pooling exchange: [warp pair][2][8][16] floats
-    const uint32_t acc_slot = pool_slot + 12u * 1024u;                            // accumulator tile: 128 rows x (n_mma + 4) floats
+    const uint32_t acc_full = b_full + 8u, acc_empty = acc_full + 32u;          // [accumulator tile][half]
+    const uint32_t abort_slot = acc_empty + 32u, tab_slot = abort_slot + 4u;
+    const uint32_t pool_slot = (tab_slot + 4u * SH_MAX_STEPS + 15u) & ~15u;      // pooling exchange: [warp pair][2][8][16] floats
+    const uint32_t acc_slot = pool_slot + 12u * 1024u;                            // accumulator tiles: acc_bufs x 128 rows x (n_mma + 4) floats
     uint8_t* gen0 = smem_raw + (base - smem_u32(smem_raw));
     const AccTile acc_tile = {reinterpret_cast<float*>(gen0 + (acc_slot - base)), p.n_mma + 4};
     volatile uint32_t* abort_g = reinterpret_cast<volatile uint32_t*>(gen0 + (abort_slot - base));
-    uint32_t* tap_tab = reinterpret_cast<uint32_t*>(gen0 + (tab_slot - base));   // per tap pair: shift | lbo << 16
+    uint32_t* tap_tab = reinterpret_cast<uint32_t*>(gen0 + (tab_slot - base));   // per K = 16 step: shift | lbo << 16
 
     const int tid = threadIdx.x, lane = tid & 31;
     const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);       // warp-uniform for the compiler (see elect_one_sync)
-    if (tid < p.n_pairs) {       // descriptor increments of every tap pair (no divisions in the issue loop)
-        const int khw = p.KH * p.KW, t0 = 2 * tid, t1 = 2 * tid + 1;
-        const int sh0 = (t0 / p.KW) * p.W + (t0 % p.KW);
-        const int sh1 = t1 < khw ? (t1 / p.KW) * p.W + (t1 % p.KW) : sh0 + 1;          // padding tap: zero weights
-        tap_tab[tid] = (uint32_t)sh0 | ((uint32_t)(sh1 - sh0) << 16);
+    if (tid < p.n_steps) {       // descriptor of every K = 16 step (kernel row kh, planes 2 u and 2 u + 1), in 16-byte units
+        const int half = p.n_planes >> 1, kh = tid / half, u = tid - kh * half, plane = p.a_plane >> 4;
+        tap_tab[tid] = (uint32_t)(2 * u * plane + kh * p.W) | ((uint32_t)plane << 16);
     }
     if (tid == 0) {
         for (int s = 0; s < SH_STAGES; ++s) { mbar_init(a_full + 8 * s, 1); mbar_init(a_empty + 8 * s, 1); }
         mbar_init(b_full, 1);
-        for (int h = 0; h < 2; ++h) {
+        for (int h = 0; h < 4; ++h) {
             mbar_init(acc_full + 8 * h, 4);                         // the MMA warps
             mbar_init(acc_empty + 8 * h, SH_EPI_WARPS / 2);         // the epilogue warps that read the half
         }
         *abort_g = 0;
         fence_mbar_init();
     }
-    {   // the A ring starts as zeros: positions past the end of the pack are never loaded, and the padding tap of an
-        // odd tap count multiplies whatever lies there by a zero weight row -- it has to be finite
+    {   // the A ring starts as zeros: positions past the end of the image are never loaded, yet feed (dropped) virtual
+        // outputs -- they have to be finite
         uint4* az = reinterpret_cast<uint4*>(gen0 + (a_base - base));
         const int n16 = SH_STAGES * p.a_stage / 16;
         for (int i = tid; i < n16; i += SH_THREADS) az[i] = make_uint4(0, 0, 0, 0);
@@ -785,7 +791,8 @@ k_conv_shift(const ShiftP p) {
         int i = 0;
         for (int t = blockIdx.x; t < p.n_tiles; t += gridDim.x) {
             if (!shift_tile_live(p, t)) continue;
-            if (!mbar_wait(acc_full + 8 * h, (uint32_t)i & 1u)) { *abort_g = 5; break; }     // this half's accumulators are in the tile
+            const int buf = p.acc_bufs > 1 ? (i & 1) : 0;
+            if (!mbar_wait(acc_full + 8 * (2 * buf + h), (uint32_t)(i / p.acc_bufs) & 1u)) { *abort_g = 5; break; }     // this half's accumulators are in the tile
             if (*abort_g) break;
             if (stamp) shift_dbg(p, i, 3 + 2 * h);
             int b, ih, iw;
@@ -807,7 +814,7 @@ k_conv_shift(const ShiftP p) {
             const size_t out_row = (size_t)b * p.Cout * ohw + pix;
             float* const out_main = (NOISY ? p.y_noisy : p.y) + out_row;
             float* const out_y = (NOISY && p.y) ? p.y + out_row : nullptr;
-            const uint32_t t_lane = (uint32_t)(q * 32) << 16;
+            const uint32_t t_lane = (uint32_t)(128 * buf + q * 32) << 16;
             if (POOL) {
                 // Fused MaxPool2d(2,2) on block tiles: the window of lane l is {l, l^1, l^8, l^9} (columns iw, iw+1 of rows
                 // ih, ih+1).  The four lanes of a window SHARE the work: the lane at window position w finalizes channel w of
@@ -961,7 +968,8 @@ k_conv_shift(const ShiftP p) {
             }
             }
             __syncwarp();
-            if (elect_one_sync()) mbar_arrive(acc_empty + 8 * h);        // this warp's rows of the half may be overwritten
+            // this warp's rows of the half may be overwritten (t_lane holds the tile: rows 128 buf + 32 q)
+            if (elect_one_sync()) mbar_arrive(acc_empty + 8 * (2 * (t_lane >> 23) + h));
             __syncwarp();
             if (stamp) shift_dbg(p, i, 4 + 2 * h);
             ++i;
@@ -1045,6 +1053,31 @@ k_pack_act(const float* __restrict__ x, __nv_bfloat16* __restrict__ xp, int B, i
     }
 }
 
+// Activations -> the row-plane image of the shift kernel ([plane][B][H][W][8]: element j of plane q at pixel (b, h, w) is
+// x[b, c, h, w + kw] for kw Cin + c = 8 q + j; zero past the right edge and past KW Cin), codes as k_pack_act
+__global__ void __launch_bounds__(256)
+k_pack_act_rows(const float* __restrict__ x, __nv_bfloat16* __restrict__ xp, int B, int C, int H, int W, int KW, int planes,
+                float code_scale) {
+    const int64_t npix = (int64_t)B * H * W, total = npix * planes;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t pixel = i % npix;
+        const int q = (int)(i / npix);
+        const int b = (int)(pixel / ((int64_t)H * W)), r = (int)(pixel - (int64_t)b * H * W), w = r % W;
+        __align__(16) __nv_bfloat16 v[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int k = q * 8 + j, kw = k / C, c = k - kw * C;
+            float f = 0.f;
+            if (kw < KW && w + kw < W) {
+                f = __ldg(x + ((int64_t)b * C + c) * H * W + r + kw);
+                if (code_scale > 0.f) f = rintf(__fdiv_rn(f, code_scale));
+            }
+            v[j] = __float2bfloat16_rn(f);
+        }
+        *reinterpret_cast<uint4*>(xp + i * 8) = *reinterpret_cast<const uint4*>(v);
+    }
+}
+
 // Weights -> pre-swizzled smem image.  mode 0 (forward): rows [main | sigma | wsum], k = tap*Cp + c reads
 // w[n][c][tap].  mode 1 (dgrad): "output channel" r = input channel c_in, k = tap'*Cp + n with the taps
 // flipped: reads w[n][r][KHW-1-tap'] (Cp = padded Cout).
@@ -1053,7 +1086,8 @@ struct PackWP {
     __nv_bfloat16* wp;
     int Cout, Cin, KHW, Cp, n_t, n_mma, num_kb, n_tiles;
     int main_col, sig_col, wsum_col, noise_mode, mode;
-    int layout;                    // 0: swizzled [tile][k-block] images, 1: shift-GEMM [k chunk][row][8] (num_kb = chunks)
+    int layout;                    // 0: swizzled [tile][k-block] images, 1: shift-GEMM [kh][plane][row][8] (num_kb = KH x planes)
+    int sh_kw, sh_planes;          // layout 1: kernel width and planes (K chunk q of kernel row kh holds k = kw Cin + c in 8 q .. 8 q + 7)
     float w_code_scale;
     // optional in-register weight quantizer (hardware_model.py:323, :343; range [-q_hi, q_hi] symmetric): the
     // main rows are then produced from w_raw directly -- k = rne(clamp((w + q_hi)/s + u, 0, qmax)), stored as the
@@ -1122,7 +1156,7 @@ __device__ __forceinline__ void pack_w_job(const PackWP& p, int64_t start, int64
                     (int64_t)rank * (p.t_nhalf * 2 * (wa + wb)) + (slot ? p.t_nhalf * 2 * wa : 0) + (int64_t)rr * (2 * w) + ((j ^ swz) << 4);
             kb = 0; kbase = 0;
         } else if (shift) {
-            r = (int)(i % p.n_mma); kb = (int)(i / p.n_mma); j = 0; tile = 0; kbase = kb * 8;
+            r = (int)(i % p.n_mma); kb = (int)(i / p.n_mma); j = 0; tile = 0; kbase = 0;
         } else {
             // Thread -> 16-byte chunk, enumerated so that a warp READS contiguous parameters (the kernel was bound by
             // 4-byte loads 100 B apart: one sector per lane): the parameter tensor is [n][c][tap] with tap fastest, so
@@ -1154,11 +1188,16 @@ __device__ __forceinline__ void pack_w_job(const PackWP& p, int64_t start, int64
         else if (p.wsum_col >= 0 && r == p.wsum_col) { kind = 2; }
         const int nrows = p.mode == 0 ? p.Cout : p.Cin;   // number of real "output" rows
         const int kdim = p.mode == 0 ? p.Cin : p.Cout;    // real channels inside a tap
-        const int tap = tma ? tap_t : kbase / p.Cp;                     // Cp % 8 == 0: a chunk never straddles taps
-        const int c_first = tma ? c_first_t : kbase - tap * p.Cp;
+        const int tap0 = tma ? tap_t : kbase / p.Cp;                    // Cp % 8 == 0: a chunk never straddles taps
+        const int c_first = tma ? c_first_t : kbase - tap0 * p.Cp;
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
-            const int c = c_first + e;
+            int tap = tap0, c = c_first + e;
+            if (shift) {        // k = kw Cin + c of kernel row kh; past KW Cin: zero
+                const int kh = kb / p.sh_planes, k = (kb - kh * p.sh_planes) * 8 + e, kw = k / p.Cin;
+                tap = kw < p.sh_kw ? kh * p.sh_kw + kw : p.KHW;
+                c = k - kw * p.Cin;
+            }
             float f = 0.f;
             if (tap < p.KHW && c < kdim && kind >= 0) {
                 if (kind == 2) {
@@ -1749,37 +1788,55 @@ static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; 
 
 // ---- shift-GEMM forward (k_conv_shift): eligibility and sizes
 struct ShiftPlan {
-    int n_t, n_mma, main_col, sig_col, n_chunks, n_pairs, a_pixels, a_stage, b_bytes, n_tiles;
+    int n_t, n_mma, main_col, sig_col, n_planes, n_chunks, n_steps, a_pixels, a_plane, a_stage, b_bytes, n_tiles, acc_bufs;
     size_t smem_bytes, wp_bytes;
 };
 int g_shift_enable = 1;        // test hook: nn_debug_shift_enable
+
+// planes of the row-plane image: K = KW * Cin of a kernel row in whole K = 16 steps of two 8-element planes
+static inline int shift_planes(int Cin, int KW) { return 2 * ((KW * Cin + 15) / 16); }
+
+// the weight image [kh][plane][row][8] (nn_prepare_weights sizes it from the same fields)
+static void shift_weight_plan(int Cin, int KH, int KW, int Cout, bool noisy, ShiftPlan* sp) {
+    sp->n_t = pad_to(Cout, 8);
+    sp->main_col = 0;
+    sp->sig_col = noisy ? sp->n_t : -1;
+    sp->n_mma = pad_to(noisy ? 2 * sp->n_t : sp->n_t, 16);
+    sp->n_planes = shift_planes(Cin, KW);
+    sp->n_chunks = KH * sp->n_planes;
+    sp->n_steps = sp->n_chunks / 2;
+    sp->b_bytes = sp->n_chunks * sp->n_mma * 16;
+    sp->wp_bytes = (size_t)sp->b_bytes;
+}
 
 static bool make_shift_plan(const nn_conv_geom& g, bool noisy, ShiftPlan* out) {
     if (!g_shift_enable) return false;
     if (g.Cin > 8 || g.stride != 1 || g.pad != 0 || g.KH > g.H || g.KW > g.W || g.W >= 4096) return false;
     if ((int64_t)g.B * g.H * g.W >= (int64_t)1 << 31) return false;
     ShiftPlan sp;
-    sp.n_t = pad_to(g.Cout, 8);
-    sp.main_col = 0;
-    sp.sig_col = noisy ? sp.n_t : -1;
-    sp.n_mma = pad_to(noisy ? 2 * sp.n_t : sp.n_t, 16);
-    if (sp.n_mma > SH_MAX_N) return false;
-    const int khw = g.KH * g.KW;
-    sp.n_pairs = (khw + 1) / 2;
-    sp.n_chunks = 2 * sp.n_pairs;
-    sp.a_pixels = UM_BLOCK_M + (g.KH - 1) * g.W + (g.KW - 1) + 8;
-    sp.a_stage = pad_to(sp.a_pixels * 16, 128);
-    sp.b_bytes = sp.n_chunks * sp.n_mma * 16;
+    shift_weight_plan(g.Cin, g.KH, g.KW, g.Cout, noisy, &sp);
+    if (sp.n_mma > SH_MAX_N || sp.n_steps > SH_MAX_STEPS) return false;
+    // pixels per plane of an A stage: 128 positions and KH - 1 rows below them (the horizontal halo is inside K); the
+    // block tiles of the pooled launches need 16 + KH - 1 image rows from the tile's column on -- the ring is sized for both
+    sp.a_pixels = UM_BLOCK_M + (g.KH - 1) * g.W;
+    const int a_pixels_blk = (15 + g.KH - 1) * g.W + 8;
+    sp.a_plane = pad_to((a_pixels_blk > sp.a_pixels ? a_pixels_blk : sp.a_pixels) * 16, 128);
+    sp.a_stage = sp.n_planes * sp.a_plane;
     sp.n_tiles = (int)(((int64_t)g.B * g.H * g.W + UM_BLOCK_M - 1) / UM_BLOCK_M);
-    // (the A ring is sized for the block tiles of the pooled launches: 16 + KH - 1 image rows)
-    const int a_stage_blk = pad_to(((15 + g.KH - 1) * g.W + 8 + (g.KW - 1) + 8) * 16, 128);
-    sp.smem_bytes = 128 + (size_t)sp.b_bytes + (size_t)SH_STAGES * (a_stage_blk > sp.a_stage ? a_stage_blk : sp.a_stage) + 16 * SH_STAGES + 96 +
-                    4 * SH_MAX_PAIRS + 16 + 12 * 1024 + (size_t)UM_BLOCK_M * (sp.n_mma + 4) * 4;
-    if (sp.n_pairs > SH_MAX_PAIRS) return false;
-    sp.wp_bytes = (size_t)sp.b_bytes;
+    const size_t acc_tile = (size_t)UM_BLOCK_M * (sp.n_mma + 4) * 4;
+    sp.smem_bytes = 128 + (size_t)sp.b_bytes + (size_t)SH_STAGES * sp.a_stage + 16 * SH_STAGES + 96 + 4 * SH_MAX_STEPS + 16 + 12 * 1024 + acc_tile;
     if (sp.smem_bytes > 227 * 1024) return false;
+    // a second accumulator tile where it fits (conv1: 222 KB): the MMA warpgroups then store a tile while the epilogue
+    // still reads the one before
+    sp.acc_bufs = sp.smem_bytes + acc_tile <= 227 * 1024 ? 2 : 1;
+    sp.smem_bytes += (sp.acc_bufs - 1) * acc_tile;
     if (out) *out = sp;
     return true;
+}
+
+// the row-plane input image of a shift launch: n_planes planes of B*H*W 16-byte pixel records
+static size_t shift_planes_bytes(const nn_conv_geom& g) {
+    return (size_t)shift_planes(g.Cin, g.KW) * g.B * g.H * g.W * 16;
 }
 
 // debug hook: per-CTA phase timestamps of the next forward launches (NN_UMMA_DEBUG=1)
@@ -1945,6 +2002,13 @@ int64_t nn_umma_fwd_workspace(const nn_conv_geom* g, int precision) {
             if (t > b) b = t;
         }
     }
+    {   // the shift kernel's row-plane image holds P >= 2 planes of the input
+        ShiftPlan sp;
+        if (make_shift_plan(*g, true, &sp) || make_shift_plan(*g, false, &sp)) {
+            const size_t t = align_up(shift_planes_bytes(*g), 1024) + align_up(sp.wp_bytes, 1024);
+            if (t > a) a = t;
+        }
+    }
     if (OH * OW == 1)          // split-K partial sums of a skinny linear forward (up to 4 shares)
         a += (size_t)4 * f.n_tiles * f.n_mma * ((g->B + UM_BLOCK_M - 1) / UM_BLOCK_M * UM_BLOCK_M) * sizeof(float) + 1024;
     return (int64_t)((a > b ? a : b) + 2048);
@@ -2000,7 +2064,7 @@ static int shift_conv_fwd(const nn_conv_fwd_args* a, const ShiftPlan& sp, int de
     int OH, OW;
     nn_out_hw(g, OH, OW);
     const bool noise = a->noise_mode != NN_NOISE_NONE;
-    const size_t xp_bytes = (size_t)g.B * g.H * g.W * 16;
+    const size_t xp_bytes = shift_planes_bytes(g);
     uint8_t* ws = (uint8_t*)align_up((size_t)a->workspace, 1024);
     const size_t need = (a->x_packed ? 0 : align_up(xp_bytes, 1024)) + (a->w_packed ? 0 : align_up(sp.wp_bytes, 1024)) + 1024;
     if ((!a->x_packed || !a->w_packed) && (!a->workspace || (size_t)a->workspace_bytes < need))
@@ -2008,10 +2072,10 @@ static int shift_conv_fwd(const nn_conv_fwd_args* a, const ShiftPlan& sp, int de
     const __nv_bfloat16* xp = (const __nv_bfloat16*)a->x_packed;
     const __nv_bfloat16* wp = (const __nv_bfloat16*)a->w_packed;
     if (!xp) {
-        const int64_t total = (int64_t)g.B * g.H * g.W;
+        const int64_t total = (int64_t)sp.n_planes * g.B * g.H * g.W;
         int grid = (int)((total + 255) / 256);
         if (grid > 16 * nn_num_sms(device)) grid = 16 * nn_num_sms(device);
-        k_pack_act<<<grid, 256, 0, st>>>(a->x, (__nv_bfloat16*)ws, g.B, g.Cin, g.H * g.W, 8, a->a_code_scale);
+        k_pack_act_rows<<<grid, 256, 0, st>>>(a->x, (__nv_bfloat16*)ws, g.B, g.Cin, g.H, g.W, g.KW, sp.n_planes, a->a_code_scale);
         NN_LAUNCH_OK();
         xp = (const __nv_bfloat16*)ws;
         ws += align_up(xp_bytes, 1024);
@@ -2022,6 +2086,7 @@ static int shift_conv_fwd(const nn_conv_fwd_args* a, const ShiftPlan& sp, int de
         pw.w_eff = a->w_eff; pw.w_raw = a->w_raw; pw.wp = (__nv_bfloat16*)ws;
         pw.Cout = g.Cout; pw.Cin = g.Cin; pw.KHW = g.KH * g.KW; pw.Cp = 8; pw.n_t = sp.n_t; pw.n_mma = sp.n_mma;
         pw.num_kb = sp.n_chunks; pw.n_tiles = 1; pw.main_col = sp.main_col; pw.sig_col = sp.sig_col; pw.wsum_col = -1;
+        pw.sh_kw = g.KW; pw.sh_planes = sp.n_planes;
         pw.noise_mode = a->noise_mode; pw.mode = 0; pw.layout = NN_PACK_SHIFT; pw.w_code_scale = a->w_code_scale;
         const int64_t total = (int64_t)sp.n_chunks * sp.n_mma;
         k_pack_w<<<(int)((total + 255) / 256), 256, 0, st>>>(pw);
@@ -2031,8 +2096,9 @@ static int shift_conv_fwd(const nn_conv_fwd_args* a, const ShiftPlan& sp, int de
     ShiftP p;
     memset(&p, 0, sizeof(p));
     p.H = g.H; p.W = g.W; p.OH = OH; p.OW = OW; p.KH = g.KH; p.KW = g.KW; p.Cout = g.Cout;
-    p.n_mma = sp.n_mma; p.main_col = sp.main_col; p.sig_col = sp.sig_col; p.n_pairs = sp.n_pairs;
-    p.a_pixels = sp.a_pixels; p.a_stage = sp.a_stage; p.b_bytes = sp.b_bytes; p.n_tiles = sp.n_tiles;
+    p.n_mma = sp.n_mma; p.main_col = sp.main_col; p.sig_col = sp.sig_col; p.n_steps = sp.n_steps; p.n_planes = sp.n_planes;
+    p.a_pixels = sp.a_pixels; p.a_plane = sp.a_plane; p.a_stage = sp.a_stage; p.b_bytes = sp.b_bytes; p.n_tiles = sp.n_tiles;
+    p.acc_bufs = sp.acc_bufs;
     p.total_pixels = (long long)g.B * g.H * g.W;
     p.xp = xp; p.wp = wp;
     const float as = a->a_code_scale > 0.f ? a->a_code_scale : 1.f;
@@ -2044,11 +2110,10 @@ static int shift_conv_fwd(const nn_conv_fwd_args* a, const ShiftPlan& sp, int de
     p.err_flag = nn_umma_err_flag(device);
     p.sbo_units = 8; p.zero_out = a->zero_out;
     if (p.pooled) {
-        // block tiles (16 rows x 8 columns of the input grid): one stage = the rows r0 .. r0 + 15 + KH - 1 from column c0 on
+        // block tiles (16 rows x 8 columns of the input grid): one stage plane = the rows r0 .. r0 + 15 + KH - 1 from column c0 on
         p.blk = 1; p.tiles_x = g.W / 8; p.tiles_per_img = (g.H / 16) * p.tiles_x; p.sbo_units = g.W;
         p.n_tiles = g.B * p.tiles_per_img;
-        p.a_pixels = (15 + g.KH - 1) * g.W + 8 + (g.KW - 1) + 8;
-        p.a_stage = pad_to(p.a_pixels * 16, 128);
+        p.a_pixels = (15 + g.KH - 1) * g.W + 8;
         if (a->bn_mean) {
             if (!a->bn_invstd || !a->bn_scratch) return nn_fail("nn_noisy_conv_fwd: bn_mean needs bn_invstd and bn_scratch%s", "");
             if (a->bn_eval_mode && (!a->bn_running_mean || !a->bn_running_var))
@@ -2140,6 +2205,10 @@ extern "C" int nn_conv_linear_bn_fusable(const nn_conv_geom* g, int32_t noise_mo
 }
 // [ticket | per-CTA partial sums of the pooled values]: 16 + SMs x Cout x 2 doubles (sized for 256 CTAs)
 extern "C" int64_t nn_conv_bn_scratch_bytes(int Cout) { return 16 + (int64_t)256 * Cout * 2 * sizeof(double); }
+extern "C" int64_t nn_conv_shift_planes_bytes(const nn_conv_geom* g) {
+    if (!g || g->Cin < 1 || g->Cin > 8 || g->KW < 1) return 0;
+    return (int64_t)shift_planes_bytes(*g);
+}
 extern "C" int nn_debug_shift_enable(int enable) {
     const int prev = g_shift_enable;
     if (enable >= 0) g_shift_enable = enable;
@@ -2324,13 +2393,14 @@ static Plan plan_for_job(const nn_wprep_job& jb) {
     return make_plan(jb.Cout, jb.KHW, jb.Cin, true, false, false, 0, (jb.m_rows + 127) / 128);
 }
 
-// shift-layout jobs carry the conv geometry implicitly: Cin <= 8, one chunk per tap
-static void shift_plan_for_job(const nn_wprep_job& jb, ShiftPlan* sp) {
-    const bool noisy = jb.noise_mode != NN_NOISE_NONE;
-    sp->n_t = pad_to(jb.Cout, 8); sp->main_col = 0; sp->sig_col = noisy ? sp->n_t : -1;
-    sp->n_mma = pad_to(noisy ? 2 * sp->n_t : sp->n_t, 16);
-    sp->n_pairs = (jb.KHW + 1) / 2; sp->n_chunks = 2 * sp->n_pairs;
-    sp->b_bytes = sp->n_chunks * sp->n_mma * 16; sp->wp_bytes = (size_t)sp->b_bytes;
+// shift-layout jobs carry the kernel size as KHW: the kernel is square (KH = KW = sqrt(KHW)), Cin <= 8
+static bool shift_plan_for_job(const nn_wprep_job& jb, ShiftPlan* sp, int* k_out) {
+    int k = 1;
+    while (k * k < jb.KHW) ++k;
+    if (k * k != jb.KHW || jb.Cin < 1 || jb.Cin > 8) return false;
+    shift_weight_plan(jb.Cin, k, k, jb.Cout, jb.noise_mode != NN_NOISE_NONE, sp);
+    if (k_out) *k_out = k;
+    return true;
 }
 
 // NN_PACK_TMA jobs: the plan depends on the channel counts, the tap count and the sigma rows only
@@ -2345,7 +2415,7 @@ static bool tma_plan_for_job(const nn_wprep_job& jb, TmaPlan* tp) {
 extern "C" int64_t nn_weight_pack_bytes(const nn_wprep_job* jb) {
     if (!jb) return 0;
     if (jb->layout == NN_PACK_TMA) { TmaPlan tp; return tma_plan_for_job(*jb, &tp) ? (int64_t)align_up(tp.wp_bytes, 1024) : 0; }
-    if (jb->layout == NN_PACK_SHIFT) { ShiftPlan sp; shift_plan_for_job(*jb, &sp); return (int64_t)align_up(sp.wp_bytes, 1024); }
+    if (jb->layout == NN_PACK_SHIFT) { ShiftPlan sp; return shift_plan_for_job(*jb, &sp, nullptr) ? (int64_t)align_up(sp.wp_bytes, 1024) : 0; }
     return (int64_t)align_up(plan_for_job(*jb).wp_bytes, 1024);
 }
 
@@ -2365,11 +2435,12 @@ extern "C" int nn_prepare_weights(const nn_wprep_job* jobs, int count, int devic
         if (jb.layout == NN_PACK_TMA) {
             if (jb.want_wsum || !tma_plan_for_job(jb, &tp))
                 return nn_fail("nn_prepare_weights: NN_PACK_TMA is not served for this job%s (see nn_conv_pack_layout)", "");
-        } else if (jb.layout == NN_PACK_SHIFT) {
-            if (jb.mode != 0 || jb.Cin > 8 || jb.want_wsum)
-                return nn_fail("nn_prepare_weights: NN_PACK_SHIFT needs a forward job with Cin <= 8 and no colsum row%s", "");
-            ShiftPlan sp;
-            shift_plan_for_job(jb, &sp);
+        }
+        ShiftPlan sp;
+        int sk = 0;
+        if (jb.layout == NN_PACK_SHIFT) {
+            if (jb.mode != 0 || jb.want_wsum || !shift_plan_for_job(jb, &sp, &sk))
+                return nn_fail("nn_prepare_weights: NN_PACK_SHIFT needs a forward job with Cin <= 8, a square kernel and no colsum row%s", "");
             pl.Cp = 8; pl.n_t = sp.n_t; pl.n_mma = sp.n_mma; pl.num_kb = sp.n_chunks; pl.n_tiles = 1;
             pl.main_col = sp.main_col; pl.sig_col = sp.sig_col; pl.wsum_col = -1;
         }
@@ -2379,6 +2450,7 @@ extern "C" int nn_prepare_weights(const nn_wprep_job* jobs, int count, int devic
         pw.num_kb = pl.num_kb; pw.n_tiles = pl.n_tiles; pw.main_col = pl.main_col; pw.sig_col = pl.sig_col;
         pw.wsum_col = pl.wsum_col; pw.noise_mode = jb.noise_mode; pw.mode = jb.mode; pw.w_code_scale = 0.f;
         pw.layout = jb.layout;
+        if (jb.layout == NN_PACK_SHIFT) { pw.sh_kw = sk; pw.sh_planes = sp.n_planes; }
         pw.q_bits = jb.q_bits;
         if (jb.q_bits > 0) {
             const double qmax = (double)((1u << jb.q_bits) - 1u);

@@ -1416,6 +1416,134 @@ extern "C" int nn_input_quant_pack(const float* x, void* xp, float* act, int B, 
     return 0;
 }
 
+// ------------------------------------------------------------------ input pack for the shift kernel's row-plane image
+// The first layer's input as the row-plane image of k_conv_shift (nn_conv_shift_planes_bytes): P planes [plane][B][H][W][8],
+// element j of plane q at pixel (b, h, w) = the code of x[b, c, h, w + kw] for kw C + c = 8 q + j, zero past the right
+// edge and past KW C; optionally the NHWC code image [B,H,W,8] from the same pass.  The codes are nn_input_quant_pack's:
+// same arithmetic, same Philox counter per pixel (pixel * 2, + 1 for channels 4..7), bit-identical.
+struct RowsP {
+    const float* x; __nv_bfloat16* xp; __nv_bfloat16* planes; const float* u_inject;
+    int B, C, H, W, KW, P, quant; float q_scale, q_max, stoch; nn_rng rng;
+};
+
+// Hot path (32-wide rows, C <= 4 channels: one draw per pixel; draws from the Philox stream or none): a warp owns one image
+// row, lane = column, so every load and store of the warp is one contiguous run (128 B per channel, 512 B per image), and
+// the codes of the KW - 1 pixels to the right of a lane come from its neighbours by shuffle.
+template <int C, int KW>
+__global__ void __launch_bounds__(256)
+k_quant_pack_rows32(const RowsP p) {
+    constexpr int P = 2 * ((KW * C + 15) / 16);
+    const NnRng rs = nn_rng_load(p.rng);
+    const int lane = threadIdx.x & 31;
+    const unsigned rows = (unsigned)p.B * p.H, HW = (unsigned)p.H * 32u, npix = rows * 32u;
+    const unsigned warps = (gridDim.x * blockDim.x) >> 5;
+    for (unsigned row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {     // warp-uniform
+        const unsigned pixel = row * 32u + lane, b = row / (unsigned)p.H, r = pixel - b * HW;
+        float v[C];
+#pragma unroll
+        for (int c = 0; c < C; ++c) v[c] = __ldg(p.x + ((size_t)b * C + c) * HW + r);
+        uint32_t rr[4] = {0u, 0u, 0u, 0u};
+        if (p.stoch > 0.f) {
+            const uint4 rnd = nn_philox(rs, (uint64_t)pixel * 2);
+            rr[0] = rnd.x; rr[1] = rnd.y; rr[2] = rnd.z; rr[3] = rnd.w;
+        }
+        float cd[C];
+#pragma unroll
+        for (int c = 0; c < C; ++c) cd[c] = quant_code(v[c], p.q_scale, p.q_max, p.stoch > 0.f ? nn_usym(rr[c], p.stoch) : 0.f);
+        if (p.xp) {
+            __align__(16) __nv_bfloat16 out[8];
+#pragma unroll
+            for (int c = 0; c < 8; ++c) out[c] = __float2bfloat16_rn(c < C ? cd[c] : 0.f);
+            *reinterpret_cast<uint4*>(p.xp + (size_t)pixel * 8) = *reinterpret_cast<const uint4*>(out);
+        }
+#pragma unroll
+        for (int q = 0; q < P; ++q) {
+            __align__(16) __nv_bfloat16 out[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int e = 8 * q + j, kw = e / C, c = e - kw * C;
+                float f = 0.f;
+                if (kw < KW) {
+                    f = __shfl_down_sync(0xffffffffu, cd[c], kw);
+                    if (lane + kw >= 32) f = 0.f;                      // past the right edge of the row
+                }
+                out[j] = __float2bfloat16_rn(f);
+            }
+            *reinterpret_cast<uint4*>(p.planes + ((size_t)q * npix + pixel) * 8) = *reinterpret_cast<const uint4*>(out);
+        }
+    }
+}
+
+// the code of channel c at pixel (b, r) of the input: quantized from x as k_quant_pack_input, or read from the NHWC code
+// image when x is NULL
+__device__ __forceinline__ float rows_code(const RowsP& p, const NnRng& rs, unsigned pixel, int b, int r, int c) {
+    if (!p.x) return __bfloat162float(p.xp[(size_t)pixel * 8 + c]);
+    const int64_t o = ((int64_t)b * p.C + c) * (p.H * p.W) + r;
+    const float v = __ldg(p.x + o);
+    if (!p.quant) return v;
+    float u = 0.f;
+    if (p.stoch > 0.f) {
+        if (p.u_inject) u = __ldg(p.u_inject + o);
+        else {
+            const uint4 rnd = nn_philox(rs, (uint64_t)pixel * 2 + (c >> 2));
+            const uint32_t rr[4] = {rnd.x, rnd.y, rnd.z, rnd.w};
+            u = nn_usym(rr[c & 3], p.stoch);
+        }
+    }
+    return quant_code(v, p.q_scale, p.q_max, u);
+}
+
+// every other case: a thread per pixel, each code made where it is needed
+__global__ void __launch_bounds__(256)
+k_quant_pack_rows(const RowsP p) {
+    const NnRng rs = nn_rng_load(p.rng);
+    const int HW = p.H * p.W;
+    const unsigned npix = (unsigned)p.B * HW;
+    for (unsigned pixel = blockIdx.x * blockDim.x + threadIdx.x; pixel < npix; pixel += gridDim.x * blockDim.x) {
+        const int b = (int)(pixel / (unsigned)HW), r = (int)(pixel - (unsigned)b * HW), w = r % p.W;
+        __align__(16) __nv_bfloat16 out[8];
+        if (p.x && p.xp) {
+            for (int c = 0; c < 8; ++c) out[c] = __float2bfloat16_rn(c < p.C ? rows_code(p, rs, pixel, b, r, c) : 0.f);
+            *reinterpret_cast<uint4*>(p.xp + (size_t)pixel * 8) = *reinterpret_cast<const uint4*>(out);
+        }
+        for (int q = 0; q < p.P; ++q) {
+            for (int j = 0; j < 8; ++j) {
+                const int e = 8 * q + j, kw = e / p.C, c = e - kw * p.C;
+                out[j] = __float2bfloat16_rn(kw < p.KW && w + kw < p.W ? rows_code(p, rs, pixel + kw, b, r + kw, c) : 0.f);
+            }
+            *reinterpret_cast<uint4*>(p.planes + ((size_t)q * npix + pixel) * 8) = *reinterpret_cast<const uint4*>(out);
+        }
+    }
+}
+
+extern "C" int nn_input_quant_pack_rows(const float* x, void* xp, void* planes, int B, int C, int H, int W, int KW, int q_bits,
+                                        double q_hi, float stochastic, const float* u_inject, nn_rng rng, int device, void* stream) {
+    if (!planes || (!x && !xp) || C < 1 || C > 8 || KW < 1 || KW > W || B < 1 || H < 1 || (int64_t)B * H * W >= ((int64_t)1 << 31))
+        return nn_fail("nn_input_quant_pack_rows: bad argument%s", "");
+    NN_SET_DEVICE(device);
+    double qmax = q_bits > 0 ? (double)((1u << q_bits) - 1u) : 0.0;
+    double scale = q_bits > 0 ? q_hi / qmax : 1.0;
+    if (scale < 1e-6) scale = 1e-6;
+    RowsP p;
+    p.x = x; p.xp = (__nv_bfloat16*)xp; p.planes = (__nv_bfloat16*)planes; p.u_inject = u_inject;
+    p.B = B; p.C = C; p.H = H; p.W = W; p.KW = KW; p.P = 2 * ((KW * C + 15) / 16); p.quant = q_bits > 0;
+    p.q_scale = (float)scale; p.q_max = (float)qmax; p.stoch = stochastic; p.rng = rng;
+    const int64_t npix = (int64_t)B * H * W;
+    const bool hot = x && q_bits > 0 && !u_inject && W == 32;
+    cudaStream_t st = (cudaStream_t)stream;
+#define NN_ROWS32(CC, KK)                                                                         \
+    if (hot && C == CC && KW == KK) {                                                            \
+        k_quant_pack_rows32<CC, KK><<<grid_cap(npix, device), 256, 0, st>>>(p);                  \
+        NN_LAUNCH_OK();                                                                          \
+        return 0;                                                                                \
+    }
+    NN_ROWS32(3, 5) NN_ROWS32(4, 5) NN_ROWS32(1, 5) NN_ROWS32(3, 3)
+#undef NN_ROWS32
+    k_quant_pack_rows<<<grid_cap(npix, device), 256, 0, st>>>(p);
+    NN_LAUNCH_OK();
+    return 0;
+}
+
 extern "C" int nn_head_fwd_bwd(const float* logits, const int64_t* labels, int B, int C, const float* gamma,
                                const float* beta, float* running_mean, float* running_var, float momentum, float eps,
                                float* loss_out, float* out, float* g, void* g_packed, int Cp, float* dgamma,

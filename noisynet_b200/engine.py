@@ -153,6 +153,12 @@ class NoisyNetEngine:
             buf = torch.zeros(int(self.lib.nn_weight_pack_bytes(C.byref(jb))) + 1024, dtype=torch.uint8, device=dev)
             jb.packed_out = (buf.data_ptr() + 1023) // 1024 * 1024
             self.wpack.append(buf)
+        # conv1 on the shift kernel reads its input as the row-plane image, written by the same launch as xp1 (which the
+        # conv1 weight gradient reads)
+        self.x1_planes = None
+        if self.jobs[0].layout == PACK_SHIFT:
+            self.x1_planes = bf16(int(self.lib.nn_conv_shift_planes_bytes(C.byref(self.geom[0]))) // 2)
+        self.x1_fwd = self.x1_planes if self.x1_planes is not None else self.xp1
         self.wp_fwd = [self.jobs[i].packed_out for i in range(4)]
         self.wp_dgrad = {3: self.jobs[4].packed_out, 2: self.jobs[5].packed_out, 1: self.jobs[6].packed_out}
         self.wp_dgrad_layout = {3: self.jobs[4].layout, 2: self.jobs[5].layout, 1: self.jobs[6].layout}
@@ -217,9 +223,8 @@ class NoisyNetEngine:
             for j in range(4):                                  # forward images only, round-to-nearest weights
                 self.jobs[j].stochastic, self.jobs[j].u_inject, self.jobs[j].rng = 0.0, None, Rng(0, 0, None)
             _lib.check(lib.nn_prepare_weights(self.jobs, 4, di, st), "nn_prepare_weights")
-            _lib.check(lib.nn_input_quant_pack(_p(x), _p(self.xp1), None, B, 3, 32 * 32, 8, int(a.q_a1), qh1, 0.0, None,
-                                               Rng(0, 0, None), di, st), "nn_input_quant_pack")
-            self._fwd_gemm(0, self.xp1, s1, self.y1n, self.noise_modes[0], self._absmax(0, W[0]))
+            self._input_pack(x, int(a.q_a1), qh1, 0.0, None, Rng(0, 0, None), st)
+            self._fwd_gemm(0, self.x1_fwd, s1, self.y1n, self.noise_modes[0], self._absmax(0, W[0]))
             self._stage_fwd(self.y1n, C1, H1, 1, self.pool1, self.amax1, m.bn1, "bn1", a.q_a2, qh2, self.xp2, self.xmax2,
                             act_max=am1, eval_mode=True)
             self._fwd_gemm(1, self.xp2, s2, self.y2n, self.noise_modes[1], self.xmax2)
@@ -258,6 +263,19 @@ class NoisyNetEngine:
         if hit is not None and hit[0] == w._version:
             return hit[1]
         return ops.tensor_stats(w.detach())[1:2]
+
+    def _input_pack(self, x, q_bits, q_hi, stoch, u, rng, stream, gathered=False):
+        """conv1's input codes: the NHWC image xp1 and, for the shift kernel, the row-plane image from the same pass (from
+        xp1 when ``gathered``: nn_input_gather_quant_pack has written it)"""
+        lib, B = self.lib, self.B
+        if self.x1_planes is None:
+            if not gathered:
+                _lib.check(lib.nn_input_quant_pack(_p(x), _p(self.xp1), None, B, 3, 32 * 32, 8, q_bits, q_hi, stoch, _p(u), rng,
+                                                   self.di, stream), "nn_input_quant_pack")
+            return
+        g = self.geom[0]
+        _lib.check(lib.nn_input_quant_pack_rows(None if gathered else _p(x), _p(self.xp1), _p(self.x1_planes), B, 3, 32, 32, g.KW,
+                                                q_bits, q_hi, stoch, _p(u), rng, self.di, stream), "nn_input_quant_pack_rows")
 
     def _fwd_gemm(self, idx, xp, a_cs, y_noisy, mode, scale_dev, z=None, pooled=None, argmax=None, bn=None, key=None, zero=None,
                   eval_mode=False):
@@ -412,9 +430,9 @@ class NoisyNetEngine:
                 _lib.check(lib.nn_input_gather_quant_pack(_p(x), _p(idx), B, 3, x.shape[2], x.shape[3], 32, 32, 0, 0, 0, _p(aug),
                                                           _p(self.xp1), None, 8, int(a.q_a1), qh1, stoch, _p(u), rng_in, di, stream),
                            "nn_input_gather_quant_pack")
+                self._input_pack(None, int(a.q_a1), qh1, stoch, None, Rng(0, 0, None), stream, gathered=True)
             else:
-                _lib.check(lib.nn_input_quant_pack(_p(x), _p(self.xp1), None, B, 3, 32 * 32, 8, int(a.q_a1), qh1, stoch, _p(u),
-                                                   rng_in, di, stream), "nn_input_quant_pack")
+                self._input_pack(x, int(a.q_a1), qh1, stoch, u, rng_in, stream)
 
         if self.side is not None:
             # conv1's image is needed at once; the other six (fc1 is 90 % of the bytes) are packed on the side stream
@@ -431,12 +449,12 @@ class NoisyNetEngine:
         if self.fuse_pool1:
             # conv1 + analog noise + MaxPool2d + the batch statistics of bn1 in ONE launch: the 104 MB fp32 conv output is
             # never written; the stage that follows only normalises, quantizes and packs
-            self._fwd_gemm(0, self.xp1, s1, None, self.noise_modes[0], self._absmax(0, W[0]), self._take("z"),
+            self._fwd_gemm(0, self.x1_fwd, s1, None, self.noise_modes[0], self._absmax(0, W[0]), self._take("z"),
                            pooled=self.pool1, argmax=self.amax1, bn=m.bn1, key="bn1", zero=self.xmax2)
             self._stage_fwd(self.pool1, C1, P1, 0, None, None, m.bn1, "bn1", a.q_a2, qh2, self.xp2, self.xmax2, self._take("u"), act_max=am1,
                             stats_ready=True, site=0)
         else:
-            self._fwd_gemm(0, self.xp1, s1, self.y1n, self.noise_modes[0], self._absmax(0, W[0]), self._take("z"))
+            self._fwd_gemm(0, self.x1_fwd, s1, self.y1n, self.noise_modes[0], self._absmax(0, W[0]), self._take("z"))
             self._stage_fwd(self.y1n, C1, H1, 1, self.pool1, self.amax1, m.bn1, "bn1", a.q_a2, qh2, self.xp2, self.xmax2, self._take("u"), act_max=am1,
                             site=0)
         if self.side is not None:
