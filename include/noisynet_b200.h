@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define NN_ABI_VERSION 17
+#define NN_ABI_VERSION 18
 
 /* ---- common ---------------------------------------------------------------------- */
 
@@ -259,6 +259,14 @@ typedef struct nn_conv_dgrad_args {
     int32_t w_packed_layout; /* NN_PACK_*: the layout `w_packed` was prepared in (nn_conv_dgrad_pack_layout)  */
 } nn_conv_dgrad_args;
 int nn_noisy_conv_dgrad(const nn_conv_dgrad_args* a, int device, void* stream);
+/* dgrad of a layer whose grad_output images fit in shared memory (k_dgrad_planes): each image is loaded once as
+ * zero-padded row planes and all taps read it there, instead of one im2col tile per (pixel tile, tap).  Served when
+ * nn_conv_dgrad_planes_ok(g): stride 1, square kernel, pad < K, Cout <= 128, Cin <= 120 (one n-tile), and
+ * H x (OW + 2 (K - 1 - pad)) <= 256 (NoisyNet's conv2; not the ResNet 3x3 layers).  Needs precision NN_PREC_BF16,
+ * gy_packed (NHWC, ceil8(Cout) channels), w_packed in NN_PACK_TMA (nn_prepare_weights mode 1) and no x_pre.  gx is
+ * bit-identical to nn_noisy_conv_dgrad's on the same packed operands (the same k16 groups in the same order). */
+int nn_conv_dgrad_planes_ok(const nn_conv_geom* g);
+int nn_conv_dgrad_planes(const nn_conv_dgrad_args* a, int device, void* stream);
 
 /* wgrad: gw = (gy^T * im2col(x)) * 1[w_lo <= w_raw <= w_hi]  (mask optional: the STE of the
  * weight quantizer, hardware_model.py:343 + :176-183).  Deterministic split-K. */

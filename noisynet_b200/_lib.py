@@ -8,7 +8,7 @@ import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("NN_LIB_PATH") or os.path.join(_HERE, "lib", "libnoisynet_b200.so")   # NN_LIB_PATH: instrumented debug builds
-ABI_VERSION = 17
+ABI_VERSION = 18
 
 NOISE_NONE, NOISE_MERGED, NOISE_EXTERNAL = 0, 1, 2
 PREC_FP32, PREC_TF32, PREC_BF16 = 0, 1, 2
@@ -178,6 +178,8 @@ SIGNATURES = {
     "nn_conv_shift_planes_bytes": (C.c_int64, [C.POINTER(ConvGeom)]),
     "nn_noisy_conv_fwd": (C.c_int, [C.POINTER(ConvFwdArgs), C.c_int, C.c_void_p]),
     "nn_noisy_conv_dgrad": (C.c_int, [C.POINTER(ConvDgradArgs), C.c_int, C.c_void_p]),
+    "nn_conv_dgrad_planes_ok": (C.c_int, [C.POINTER(ConvGeom)]),
+    "nn_conv_dgrad_planes": (C.c_int, [C.POINTER(ConvDgradArgs), C.c_int, C.c_void_p]),
     "nn_conv_wgrad_workspace_bytes": (C.c_int64, [C.POINTER(ConvGeom), C.c_int32, C.c_int]),
     "nn_noisy_conv_wgrad": (C.c_int, [C.POINTER(ConvWgradArgs), C.c_int, C.c_void_p]),
 }

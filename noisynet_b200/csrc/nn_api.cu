@@ -2,6 +2,7 @@
 // Validates arguments and dispatches on `precision` to the CUDA-core fp32 kernels
 // (nn_conv_simt.cu) or the tensor-core kernels (nn_conv_umma.cu, nn_conv_tma.cu).  No CPU fallback exists.
 #include "nn_common.cuh"
+#include "nn_conv_tma.h"
 
 int nn_simt_conv_fwd(const nn_conv_fwd_args* a, int device, cudaStream_t st);
 int nn_simt_conv_dgrad(const nn_conv_dgrad_args* a, int device, cudaStream_t st);
@@ -81,6 +82,21 @@ extern "C" int nn_noisy_conv_dgrad(const nn_conv_dgrad_args* a, int device, void
     if (!nn_umma_supports(&a->g, 1))
         return nn_fail("nn_noisy_conv_dgrad: geometry not supported by the tensor-core path%s; use NN_PREC_FP32", "");
     return nn_umma_conv_dgrad(a, device, (cudaStream_t)stream);
+}
+
+extern "C" int nn_conv_dgrad_planes_ok(const nn_conv_geom* g) {
+    return g && nn_dgrad_planes_plan(*g, nullptr) ? 1 : 0;
+}
+
+extern "C" int nn_conv_dgrad_planes(const nn_conv_dgrad_args* a, int device, void* stream) {
+    if (!a) return nn_fail("nn_conv_dgrad_planes: null args%s", "");
+    if (int e = check_geom(a->g, "nn_conv_dgrad_planes")) return e;
+    if (a->precision != NN_PREC_BF16 || !a->gy_packed || !a->w_packed || a->w_packed_layout != NN_PACK_TMA || !a->gx || a->x_pre)
+        return nn_fail("nn_conv_dgrad_planes: needs NN_PREC_BF16, gy_packed, an NN_PACK_TMA w_packed and gx%s, and no x_pre", "");
+    DgPlanesPlan d;
+    if (!nn_dgrad_planes_plan(a->g, &d)) return nn_fail("nn_conv_dgrad_planes: geometry not served%s (see nn_conv_dgrad_planes_ok)", "");
+    NN_SET_DEVICE(device);
+    return nn_dgrad_planes_launch(*a, d, device, (cudaStream_t)stream);
 }
 
 extern "C" int64_t nn_conv_wgrad_workspace_bytes(const nn_conv_geom* g, int32_t precision, int dev) {

@@ -341,8 +341,9 @@ TmaConvKernel tma_conv_kernel(int nt) {
 
 // once per (device, kernel): the shared-memory opt-in; once per (device, shared-memory size): the number of co-resident
 // clusters (an occupancy query of one kernel stands for all: same block size, one CTA per SM whatever the width)
-int tma_conv_prepare(TmaConvKernel kern, int device, const cudaLaunchConfig_t& cfg, int* n_cl) {
-    struct Seen { int device; TmaConvKernel kern; };
+template <typename Kernel>
+int tma_conv_prepare(Kernel kern, int device, const cudaLaunchConfig_t& cfg, int* n_cl) {
+    struct Seen { int device; Kernel kern; };
     struct Occ { int device; size_t smem; int clusters; };
     static Seen seen[256];
     static Occ occ[32];
@@ -485,6 +486,332 @@ int nn_tma_encode_rows(void* map_out, const void* ptr, uint64_t rows, uint64_t c
                            estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return nn_fail("nn_conv_tma: cuTensorMapEncodeTiled (matrix rows) failed%s (CUresult %lld)", "", (long long)r);
+    return 0;
+}
+
+// ================================================================== dgrad on a resident row-plane image of grad_output
+//   gx[b, n, oh, ow] = sum_{tap, c} gyp[b, oh + kh - pad', ow + kw - pad', c] * Wp[n, tap, c]       (pad' = K - 1 - pad)
+// k_conv_tma loads one im2col tile per (128-pixel tile, tap): 25 x 32 KB per tile for conv2's dgrad, ~600 MB of L2 -> SM
+// traffic per step to read a 12 MB grad_output.  k_dgrad_planes loads each image ONCE and takes all taps from it:
+// * A operand: the image zero-padded by pad' on every side (GH x GW pixels, 18 x 18 for conv2) as row planes -- plane q
+//   holds channels 8 q .. 8 q + 7, one 16-byte row per pixel (the SWIZZLE_NONE K-major core-matrix row).  One tiled
+//   tensor-map copy per plane (box {8, GW, GH, 1} from (8 q, -pad', -pad', b)) lands it, the TMA unit zero-filling the
+//   halo.  Outputs live on a virtual grid r = oh * GW + ow (OH x GW rows, 4 m64 blocks); tap (kh, kw) is the same planes
+//   read kh * GW + kw rows later: the descriptor's start address moves, SBO = 8 rows (128 B), LBO = the plane stride.
+//   Planes past the channels and rows past the grid that the last block's taps reach are zeroed once at kernel start.
+// * B operand: the NN_PACK_TMA dgrad image and weight maps of k_conv_tma, one ring stage per tap, each CTA of a pair
+//   multicasting one row half.
+// * Work item: one image per CTA, clusters of two CTAs on images 2 i, 2 i + 1 in lockstep (an odd last image: rank 1
+//   reloads its partner's and stores nothing).  k16 step j of a tap is channels 16 j .. 16 j + 15 and the taps run in
+//   k_conv_tma's order, so every output receives the same products in the same k16 groups in the same order: gx is
+//   bit-identical to k_conv_tma<2, NT>'s.
+// * Warp roles: warps 0-7 two MMA warpgroups (m64 blocks 2 g, 2 g + 1 each; epilogue from the fragments), warp 8 the
+//   weight ring, warp 9 the A image (refilled once both warpgroups' chains over the previous image have completed, so
+//   it lands during their epilogue; one full barrier per plane pair lets the first tap start on the first planes).
+namespace {
+
+constexpr int DP_MAX_STAGES = 8;
+constexpr int DP_MAX_PAIRS = 8;              // 16 planes: up to 128 channels
+
+struct DgPlanesP {
+    CUtensorMap map_gy;                      // tiled {Cp, W, H, B} over grad_output, box {8, GW, GH, 1}: one plane of one image
+    CUtensorMap mapb64, mapb_tail;           // the weight image as in k_conv_tma
+    int B, OH, OW, Cout, pad, KW, taps, GW, GH;
+    int n_c64, tail_w, nc, n_mma, n_half, tap_bytes;
+    int n_load, n_pairs, plane_bytes, stages, b_stage;
+    float y_scale;
+    float* gx;
+    int* err_flag;
+};
+
+// the wgmmas of one tap over m64 blocks 0 and 1 of the warpgroup (block 1: 64 rows = 64 descriptor units later): k16 step k
+// reads plane pair k (`pstep` units apart) and weight columns 16 k .. of chunk a, then of chunk b; committed as one group,
+// returning when the previous tap's group has completed.  scale_d of the first step: 0 starts the accumulators of an image.
+template <int N, int KA, int KB>
+__device__ __forceinline__ void planes_tap_mma(float* acc0, float* acc1, uint64_t ad, uint64_t pstep, uint64_t bd_a, uint64_t bd_b, int acc_in) {
+    wg_fence();
+#pragma unroll
+    for (int k = 0; k < KA + KB; ++k) {
+        const uint64_t a = ad + (uint64_t)k * pstep, b = k < KA ? bd_a + 2 * k : bd_b + 2 * (k - KA);
+        wgmma_c<N, 0, 0>(acc0, a, b, k == 0 ? acc_in : 1);
+        wgmma_c<N, 0, 0>(acc1, a + 64, b, k == 0 ? acc_in : 1);
+    }
+    wg_commit();
+    wg_wait_1();
+}
+
+template <int NT>
+__global__ void __launch_bounds__((8 + 2) * 32, 1)
+k_dgrad_planes(const __grid_constant__ DgPlanesP p) {
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    const int S = p.stages;
+    const uint32_t a_base = base + (uint32_t)S * (uint32_t)p.b_stage;
+    const uint32_t a_bytes = (uint32_t)(2 * p.n_pairs * p.plane_bytes);
+    const uint32_t bar_base = a_base + a_bytes;
+    const uint32_t full_bar = bar_base, empty_bar = bar_base + 8u * DP_MAX_STAGES;
+    const uint32_t a_full = bar_base + 16u * DP_MAX_STAGES, a_empty = a_full + 8u * DP_MAX_PAIRS;
+
+    const int tid = threadIdx.x, lane = tid & 31;
+    const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+    const uint32_t rank = cluster_ctarank(), peer = rank ^ 1u;
+    const int pairs = (p.B + 1) >> 1;
+    const int cl0 = blockIdx.x >> 1, n_cl = gridDim.x >> 1;
+    // chunk widths of a tap (one ring stage: k_conv_tma's single group of <= 128 channels)
+    const int wa = p.n_c64 > 0 ? 64 : p.tail_w;
+    const int wb = p.nc > 1 ? (p.n_c64 > 1 ? 64 : p.tail_w) : 0;
+
+    if (tid == 0) {
+        for (int s = 0; s < S; ++s) {
+            mbar_init(full_bar + 8 * s, 1);          // the weight producer's arrive.expect_tx (both row halves)
+            mbar_init(empty_bar + 8 * s, 4);         // both MMA warpgroups of both CTAs have read the stage
+        }
+        for (int j = 0; j < p.n_pairs; ++j) mbar_init(a_full + 8 * j, 1);
+        mbar_init(a_empty, 2);                       // both MMA warpgroups of this CTA are done with the image
+        fence_mbar_init();
+        tma_prefetch_desc(&p.map_gy);
+        tma_prefetch_desc(&p.mapb64);
+        tma_prefetch_desc(&p.mapb_tail);
+    }
+    {   // zeros the copies never write: rows past the padded grid of the loaded planes, and whole planes past the channels
+        const int grid_bytes = p.GH * p.GW * 16;
+        uint8_t* const a_gen = smem_raw + (a_base - smem_u32(smem_raw));
+        const int tail_bytes = p.plane_bytes - grid_bytes;
+        const int n_tail = p.n_load * (tail_bytes >> 4), n_rest = (2 * p.n_pairs - p.n_load) * (p.plane_bytes >> 4);
+        for (int i = tid; i < n_tail + n_rest; i += blockDim.x) {
+            const int off = i < n_tail ? (i / (tail_bytes >> 4)) * p.plane_bytes + grid_bytes + 16 * (i % (tail_bytes >> 4))
+                                       : p.n_load * p.plane_bytes + 16 * (i - n_tail);
+            *reinterpret_cast<uint4*>(a_gen + off) = make_uint4(0u, 0u, 0u, 0u);
+        }
+        fence_proxy_async();                         // visible to the wgmmas (async proxy)
+    }
+    cluster_sync();                                  // barriers initialised and zeros written before any copy, arrival or wgmma
+
+    if (warp == 8) {
+        // ---------------------------------------------------------------- weight ring: one stage per tap
+        int s = 0, fail = 0;
+        uint32_t eph = 1u;
+        const uint32_t half_bytes = (uint32_t)(p.n_half * 2 * (wa + wb));
+        const int h = (int)rank;                             // this CTA's row half goes to both CTAs of the pair
+        for (int pi = cl0; pi < pairs && !fail; pi += n_cl) {
+            for (int t = 0; t < p.taps; ++t) {
+                if (!mbar_wait_backoff(empty_bar + 8 * s, eph)) { fail = 601; break; }
+                if (elect_one_sync()) {
+                    const uint32_t bar = full_bar + 8 * s, b_dst = base + (uint32_t)s * (uint32_t)p.b_stage;
+                    mbar_arrive_expect_tx(bar, 2u * half_bytes);
+                    const long long boff = (long long)t * p.tap_bytes + (long long)h * half_bytes;
+                    const uint32_t da = b_dst + (uint32_t)(h * p.n_half * 2 * wa);
+                    if (wa == 64) tma_tile_2d_mc(da, &p.mapb64, bar, 0, (int)(boff >> 7), 0x3);
+                    else tma_tile_2d_mc(da, &p.mapb_tail, bar, 0, (int)(boff / (2 * wa)), 0x3);
+                    if (wb) {
+                        const long long boff2 = boff + (long long)p.n_half * 2 * wa;
+                        const uint32_t db = b_dst + (uint32_t)(p.n_mma * 2 * wa + h * p.n_half * 2 * wb);
+                        if (wb == 64) tma_tile_2d_mc(db, &p.mapb64, bar, 0, (int)(boff2 >> 7), 0x3);
+                        else tma_tile_2d_mc(db, &p.mapb_tail, bar, 0, (int)(boff2 / (2 * wb)), 0x3);
+                    }
+                }
+                __syncwarp();
+                if (++s == S) { s = 0; eph ^= 1u; }
+            }
+        }
+        if (fail) nn_pipeline_abort(p.err_flag, fail);
+        __syncwarp();
+    } else if (warp == 9) {
+        // ---------------------------------------------------------------- A image: one copy per plane, a barrier per pair
+        int fail = 0;
+        uint32_t eph = 1u;
+        const uint32_t box_bytes = (uint32_t)(p.GH * p.GW * 16);
+        for (int pi = cl0; pi < pairs; pi += n_cl) {
+            const int b = min(2 * pi + (int)rank, p.B - 1);
+            if (!mbar_wait_backoff(a_empty, eph)) { fail = 602; break; }
+            eph ^= 1u;
+            if (elect_one_sync()) {
+                for (int j = 0; j < p.n_pairs; ++j) {
+                    const int nq = max(0, min(2, p.n_load - 2 * j));
+                    mbar_arrive_expect_tx(a_full + 8 * j, (uint32_t)nq * box_bytes);
+                    for (int q = 2 * j; q < 2 * j + nq; ++q)
+                        tma_tile_4d(a_base + (uint32_t)(q * p.plane_bytes), &p.map_gy, a_full + 8 * j, 8 * q, -p.pad, -p.pad, b);
+                }
+            }
+            __syncwarp();
+        }
+        if (fail) nn_pipeline_abort(p.err_flag, fail);
+        __syncwarp();
+    } else if (warp < 8) {
+        // ---------------------------------------------------------------- MMA warpgroups + epilogue
+        const int wg = warp >> 2, wt = tid & 127;
+        const bool releaser = (warp & 3) == 0;
+        const int kt = p.tail_w >> 4;
+        const int shape = 8 * (wa == 64 ? 4 : kt) + (wb == 64 ? 4 : (wb ? kt : 0));
+        const uint32_t plane_units = (uint32_t)p.plane_bytes >> 4;
+        const uint64_t pstep = 2ull * plane_units;
+        const int ohw = p.OH * p.OW;
+        const float y_scale = p.y_scale;
+        int s = 0, prev = 0, fail = 0;
+        uint32_t fph = 0u, aph = 0u;
+        for (int pi = cl0; pi < pairs && !fail; pi += n_cl) {
+            const int b = 2 * pi + (int)rank;
+            float acc[2][NT / 2];
+            int kh = 0, kw = 0;
+            for (int t = 0; t < p.taps; ++t) {
+                if (!mbar_wait(full_bar + 8 * s, fph)) { fail = 603; break; }
+                const uint32_t b_s = base + (uint32_t)s * (uint32_t)p.b_stage;
+                const uint64_t bd_a = gmma_desc_kmajor(b_s, 2u * (uint32_t)wa);
+                const uint64_t bd_b = wb ? gmma_desc_kmajor(b_s + (uint32_t)(p.n_mma * 2 * wa), 2u * (uint32_t)wb) : 0;
+                const uint64_t ad = gmma_desc_none(a_base + 16u * (uint32_t)(128 * wg + kh * p.GW + kw), plane_units, 8u);
+                if (t == 0) {                                // the image (this item's A phase)
+                    for (int j = 0; j < p.n_pairs && !fail; ++j)
+                        if (!mbar_wait(a_full + 8 * j, aph)) fail = 604;
+                    if (fail) break;
+                }
+                const int acc_in = t != 0 ? 1 : 0;
+                // one straight-line sequence per tap shape, as in k_conv_tma
+                switch (shape) {
+                    case 8 * 4 + 4: planes_tap_mma<NT, 4, 4>(acc[0], acc[1], ad, pstep, bd_a, bd_b, acc_in); break;
+                    case 8 * 4 + 2: planes_tap_mma<NT, 4, 2>(acc[0], acc[1], ad, pstep, bd_a, bd_b, acc_in); break;
+                    case 8 * 4 + 1: planes_tap_mma<NT, 4, 1>(acc[0], acc[1], ad, pstep, bd_a, bd_b, acc_in); break;
+                    case 8 * 4: planes_tap_mma<NT, 4, 0>(acc[0], acc[1], ad, pstep, bd_a, bd_b, acc_in); break;
+                    case 8 * 2: planes_tap_mma<NT, 2, 0>(acc[0], acc[1], ad, pstep, bd_a, bd_b, acc_in); break;
+                    default: planes_tap_mma<NT, 1, 0>(acc[0], acc[1], ad, pstep, bd_a, bd_b, acc_in); break;
+                }
+                if (t != 0 && releaser && elect_one_sync()) {      // the previous tap's weights may be refilled
+                    mbar_arrive(empty_bar + 8 * prev);
+                    mbar_arrive_cluster(cluster_map(empty_bar + 8 * prev, peer));
+                }
+                __syncwarp();
+                prev = s;
+                if (++kw == p.KW) { kw = 0; ++kh; }
+                if (++s == S) { s = 0; fph ^= 1u; }
+            }
+            if (fail) break;
+            wg_wait_all();
+            wg_fence_regs<NT / 2>(acc[0]);
+            wg_fence_regs<NT / 2>(acc[1]);
+            if (releaser && elect_one_sync()) {
+                mbar_arrive(empty_bar + 8 * prev);
+                mbar_arrive_cluster(cluster_map(empty_bar + 8 * prev, peer));
+                mbar_arrive(a_empty);                        // the next image may land while this one's outputs are stored
+            }
+            __syncwarp();
+            aph ^= 1u;
+            if (b >= p.B) continue;                          // rank 1's copy of an odd last image: nothing to store
+            // ---- epilogue from the fragments: virtual row r -> (oh, ow) = (r / GW, r % GW), real where ow < OW, oh < OH
+            float* const out = p.gx + (size_t)b * p.Cout * ohw;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = 128 * wg + 64 * i + 16 * (wt >> 5) + (lane >> 2) + 8 * h;
+                    const int oh = r / p.GW, ow = r - oh * p.GW;
+                    if (oh >= p.OH || ow >= p.OW) continue;
+                    float* const o = out + oh * p.OW + ow;
+#pragma unroll
+                    for (int ii = 0; ii < NT / 8; ++ii) {
+#pragma unroll
+                        for (int j = 0; j < 2; ++j) {
+                            const int n = 8 * ii + 2 * (lane & 3) + j;
+                            if (n < p.Cout) o[(size_t)n * ohw] = acc[i][4 * ii + 2 * h + j] * y_scale;
+                        }
+                    }
+                }
+            }
+        }
+        if (fail) nn_pipeline_abort(p.err_flag, fail);
+    }
+    cluster_sync();                                  // neither CTA exits while its peer can still write to it or arrive on it
+}
+
+typedef void (*DgPlanesKernel)(const DgPlanesP);
+
+// k_dgrad_planes<NT> for NT = nt (multiples of 8 up to NMAX)
+template <int NT, int NMAX>
+DgPlanesKernel dgrad_planes_kernel(int nt) {
+    if (nt == NT) return k_dgrad_planes<NT>;
+    if constexpr (NT + 8 <= NMAX) return dgrad_planes_kernel<NT + 8, NMAX>(nt);
+    else return nullptr;
+}
+
+}  // namespace
+
+bool nn_dgrad_planes_plan(const nn_conv_geom& g, DgPlanesPlan* out) {
+    if (g.stride != 1 || g.KH != g.KW || g.pad > g.KH - 1 || g.Cout > 128) return false;
+    DgPlanesPlan d;
+    memset(&d, 0, sizeof(d));
+    d.pad = g.KH - 1 - g.pad;
+    if (!nn_tma_make_plan(g.Cout, g.KH, g.KW, 1, d.pad, g.Cin, false, g.H, g.W, &d.tp)) return false;
+    const TmaPlan& tp = d.tp;
+    if (tp.n_tiles != 1 || tp.n_t > 120 || tp.gpt != 1) return false;
+    int OH, OW;                                      // grad_output
+    nn_out_hw(g, OH, OW);
+    d.GW = OW + 2 * d.pad;
+    d.GH = OH + 2 * d.pad;
+    if (g.H * d.GW > 256 || d.GH > 256) return false;       // four m64 blocks of virtual rows; one tensor-map box per plane
+    const int reach = 256 + (g.KH - 1) * (d.GW + 1);        // rows the last block's last tap reads
+    d.rows = tc_pad_to(d.GH * d.GW > reach ? d.GH * d.GW : reach, 8);
+    d.n_planes = tp.wt / 8;
+    d.n_load = tp.Cp / 8;
+    d.plane_bytes = d.rows * 16;
+    const int a_bytes = d.n_planes * d.plane_bytes;
+    d.stages = (222 * 1024 - 2048 - a_bytes) / tp.b_stage;
+    if (d.stages > DP_MAX_STAGES) d.stages = DP_MAX_STAGES;
+    if (d.stages < 2) return false;
+    d.smem_bytes = 1024 + (size_t)d.stages * tp.b_stage + a_bytes + 8 * (2 * DP_MAX_STAGES + DP_MAX_PAIRS + 1);
+    if (out) *out = d;
+    return true;
+}
+
+int nn_dgrad_planes_launch(const nn_conv_dgrad_args& a, const DgPlanesPlan& d, int device, cudaStream_t st) {
+    const TmaPlan& pl = d.tp;
+    const nn_conv_geom& g = a.g;
+    int OH, OW;
+    nn_out_hw(g, OH, OW);
+    DgPlanesP p;
+    memset(&p, 0, sizeof(p));
+    {   // grad_output [B][OH][OW][Cp] bf16: boxes of one plane (8 channels) of the zero-padded GH x GW grid of one image
+        EncodeTiledFn enc = get_encode_tiled();
+        if (!enc) return nn_fail("nn_conv_tma: cuTensorMapEncodeTiled is not available%s", "");
+        const cuuint64_t Cp = (cuuint64_t)pl.Cp;
+        cuuint64_t dims[4] = {Cp, (cuuint64_t)OW, (cuuint64_t)OH, (cuuint64_t)g.B};
+        cuuint64_t strides[3] = {Cp * 2, (cuuint64_t)OW * Cp * 2, (cuuint64_t)OH * OW * Cp * 2};
+        cuuint32_t box[4] = {8, (cuuint32_t)d.GW, (cuuint32_t)d.GH, 1};
+        cuuint32_t estr[4] = {1, 1, 1, 1};
+        const CUresult r = enc(&p.map_gy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(a.gy_packed), dims, strides, box, estr,
+                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) return nn_fail("nn_conv_dgrad_planes: cuTensorMapEncodeTiled (grad_output planes) failed%s (CUresult %lld)", "",
+                                              (long long)r);
+    }
+    if (((uintptr_t)a.w_packed & 15) != 0) return nn_fail("nn_conv_dgrad_planes: the weight image must be 16-byte aligned%s", "");
+    if (pl.n_c64 > 0) { if (int e = encode_weight_map(&p.mapb64, a.w_packed, pl.wp_bytes, 64, pl.n_half)) return e; }
+    if (pl.tail_w > 0) { if (int e = encode_weight_map(&p.mapb_tail, a.w_packed, pl.wp_bytes, pl.tail_w, pl.n_half)) return e; }
+    if (pl.n_c64 == 0) p.mapb64 = p.mapb_tail;
+    if (pl.tail_w == 0) p.mapb_tail = p.mapb64;
+    p.B = g.B; p.OH = g.H; p.OW = g.W; p.Cout = g.Cin; p.pad = d.pad; p.KW = g.KW; p.taps = pl.taps; p.GW = d.GW; p.GH = d.GH;
+    p.n_c64 = pl.n_c64; p.tail_w = pl.tail_w; p.nc = pl.nc; p.n_mma = pl.n_mma; p.n_half = pl.n_half; p.tap_bytes = pl.tap_bytes;
+    p.n_load = d.n_load; p.n_pairs = d.n_planes / 2; p.plane_bytes = d.plane_bytes; p.stages = d.stages; p.b_stage = pl.b_stage;
+    p.y_scale = a.w_code_scale > 0.f ? a.w_code_scale : 1.f;
+    p.gx = a.gx; p.err_flag = nn_umma_err_flag(device);
+    const DgPlanesKernel kern = dgrad_planes_kernel<8, 120>(pl.n_t);
+    if (!kern) return nn_fail("nn_conv_dgrad_planes: no kernel for an n-tile of%s %lld columns", "", (long long)pl.n_t);
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.blockDim = dim3((8 + 2) * 32);
+    cfg.dynamicSmemBytes = d.smem_bytes;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int n_cl = 0;
+    if (int e = tma_conv_prepare(kern, device, cfg, &n_cl)) return e;
+    const int pairs = (g.B + 1) / 2;
+    if (n_cl > pairs) n_cl = pairs;
+    cfg.gridDim = dim3(2 * n_cl);
+    NN_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, p));
+    NN_LAUNCH_OK();
     return 0;
 }
 

@@ -36,6 +36,21 @@ struct TmaConvCall {
 };
 int nn_tma_conv_launch(const TmaConvCall& c, int device, cudaStream_t st);
 
+// ---- dgrad on a resident row-plane image of grad_output (k_dgrad_planes): stride 1, square kernels, <= 128 grad_output
+// channels, one n-tile of <= 120 columns, the dgrad output on a virtual grid of <= 256 rows (OH x the padded width GW)
+struct DgPlanesPlan {
+    TmaPlan tp;                 // the k_conv_tma dgrad plan: weight image, chunk widths, n-tile
+    int pad;                    // K - 1 - pad of the layer: the zero halo around each grad_output image
+    int GW, GH, rows;           // padded grid (GH x GW pixels) and the rows of a plane (grid + what the last taps reach)
+    int n_planes, n_load;       // planes the k16 steps read (16-byte rows = 8 channels) / planes the copies fill
+    int plane_bytes, stages;
+    size_t smem_bytes;
+};
+bool nn_dgrad_planes_plan(const nn_conv_geom& g, DgPlanesPlan* out);
+// a: the layer's dgrad call with gy_packed (NHWC, ceil8(Cout) channels) and an NN_PACK_TMA w_packed, checked by the caller
+int nn_dgrad_planes_launch(const nn_conv_dgrad_args& a, const DgPlanesPlan& d, int device, cudaStream_t st);
+int* nn_umma_err_flag(int device);
+
 // ---- weight gradient with TMA-staged operands (k_wgrad_tma): the (tap, 64-channel chunk) columns of the gradient
 struct TmaWgradPlan {
     int Cp, Coutp, taps, n_c64, tail_w;        // tail_w: 0 or 8 channels per tap (the remainder launch)

@@ -93,6 +93,10 @@ __device__ __forceinline__ void tma_tile_2d(uint32_t dst, const void* map, uint3
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
+__device__ __forceinline__ void tma_tile_4d(uint32_t dst, const void* map, uint32_t bar, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+                 ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
 // One lane of a CONVERGED warp.  The single-thread instructions of this file (TMA copies, barrier arrivals) take
 // their operands from uniform registers; issued under `if (lane == 0)` inside divergent code the compiler cannot prove the
 // operands warp-uniform and moves every one of them through R2UR in an ELECT loop on each use (5 per MMA, ~250 cycles per

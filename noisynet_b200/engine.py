@@ -23,7 +23,7 @@ import os
 import torch
 
 from . import _lib, ops
-from ._lib import (NOISE_EXTERNAL, NOISE_MERGED, PACK_SHIFT, PREC_BF16, ConvDgradArgs, ConvFwdArgs, ConvGeom, ConvWgradArgs,
+from ._lib import (NOISE_EXTERNAL, NOISE_MERGED, PACK_SHIFT, PACK_TMA, PREC_BF16, ConvDgradArgs, ConvFwdArgs, ConvGeom, ConvWgradArgs,
                    Rng, StageArgs, StageBwdArgs, TailArgs, WPrepJob)
 from .hardware_model import _f32
 
@@ -162,6 +162,9 @@ class NoisyNetEngine:
         self.wp_fwd = [self.jobs[i].packed_out for i in range(4)]
         self.wp_dgrad = {3: self.jobs[4].packed_out, 2: self.jobs[5].packed_out, 1: self.jobs[6].packed_out}
         self.wp_dgrad_layout = {3: self.jobs[4].layout, 2: self.jobs[5].layout, 1: self.jobs[6].layout}
+        # conv2's dgrad on the resident row-plane kernel: each grad_output image loaded once for all 25 taps (the same
+        # NN_PACK_TMA image and bit-identical gx); nn_noisy_conv_dgrad serves geometries it does not
+        self.dgrad_planes = self.jobs[6].layout == PACK_TMA and bool(self.lib.nn_conv_dgrad_planes_ok(C.byref(self.geom[1])))
         need = 0
         for g in self.geom + [self.geom_fc1_lin]:
             need = max(need, self.lib.nn_conv_workspace_bytes(C.byref(g), PREC_BF16),
@@ -332,7 +335,10 @@ class NoisyNetEngine:
         a.w_packed_layout = self.wp_dgrad_layout[layer]
         a.precision, a.w_code_scale = PREC_BF16, self.w_cs[layer]
         a.workspace, a.workspace_bytes = _p(self.ws), self.ws.numel()
-        _lib.check(self.lib.nn_noisy_conv_dgrad(C.byref(a), self.di, self._st()), "nn_noisy_conv_dgrad")
+        if layer == 1 and self.dgrad_planes:
+            _lib.check(self.lib.nn_conv_dgrad_planes(C.byref(a), self.di, self._st()), "nn_conv_dgrad_planes")
+        else:
+            _lib.check(self.lib.nn_noisy_conv_dgrad(C.byref(a), self.di, self._st()), "nn_noisy_conv_dgrad")
 
     def _stage_fwd(self, x_in, C_, H, pool, pooled, amax, bn, key, q_bits, q_hi, xp, xmax, u=None, act_max=None, eval_mode=False,
                    stats_ready=False, site=None):
