@@ -198,7 +198,8 @@ typedef struct nn_conv_fwd_args {
 int64_t nn_conv_bn_scratch_bytes(int Cout);
 /* bn_mean is also served for LINEAR layers whose launch is split over K (fully connected layers at training batch sizes:
  * the split-K epilogue adds the per-channel sums; BatchNorm1d, noisynet.py:540-546): 1 if this geometry qualifies.  There
- * bn_scratch is nn_stage_scratch_bytes(Cout) bytes (the stage kernels' scratch can be shared), zeroed once. */
+ * bn_scratch is nn_stage_scratch_bytes(Cout) bytes, zeroed once, and belongs to this launch alone: the split-K epilogue
+ * lays its partial sums and counters out differently from the stage kernels, so it must not share their scratch. */
 int nn_conv_linear_bn_fusable(const nn_conv_geom* g, int32_t noise_mode, int32_t precision, int device);
 
 /* Packed-weight layouts.  NN_PACK_TILED: 128B-swizzled [n-tile][k-block] shared-memory images (every geometry).
@@ -341,8 +342,10 @@ typedef struct nn_stage_args {
     void* xp; int32_t Cp;     /* out [B,H',W',Cp] bf16 codes, Cp % 8 == 0                            */
     float* act;               /* optional out: dequantised activation, NCHW fp32                      */
     float* xmax_out;          /* optional out: max of the activation (device scalar)                  */
-    void* scratch;            /* nn_stage_scratch_bytes(C) bytes, ZEROED once by the caller (kernels keep it
-                                 consistent); shared by the forward and backward of all stages          */
+    void* scratch;            /* at least nn_stage_scratch_bytes(C) bytes, ZEROED once by the caller (kernels keep it
+                                 consistent): per-channel records of partial sums and an arrival counter, at
+                                 addresses independent of C.  One scratch sized for the widest stage may serve the
+                                 forward and backward of every stage, launched in order on one stream           */
     int32_t eval_mode;        /* 1: model.eval() -- BatchNorm normalises with running_mean / running_var and updates
                                  nothing (noisynet.py:1560-1567); the caller passes stochastic = 0 (hardware_model.py:283-286) */
     int32_t stats_ready;      /* 1: mean / invstd (and the running statistics, and *xmax_out = 0) were already produced by

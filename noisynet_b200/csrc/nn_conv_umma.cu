@@ -66,7 +66,7 @@ struct UmmaP {
     int a_tma;                     // linear layers (the im2col row of sample m is row m of a row-major matrix): A by ONE tensor-map copy
     // optional (split-K linear layers): BatchNorm batch statistics of the output from the split-K epilogue (nn_conv_fwd_args.bn_mean)
     BnFinP bn_fin;                 // bn_fin.mean != nullptr selects it
-    void* bn_scratch;              // nn_stage_scratch_bytes(Cout): [Cout][16][2] double partial sums, then [Cout] arrival counters
+    void* bn_scratch;              // nn_stage_scratch_bytes(Cout) bytes: [Cout][16][2] double partial sums, then [Cout] arrival counters
     float* zero_out;
 };
 struct UmmaAMap { alignas(64) unsigned char bytes[128]; };      // CUtensorMap of the activation matrix (a_tma)

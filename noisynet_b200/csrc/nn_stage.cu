@@ -35,23 +35,31 @@ __device__ __forceinline__ float quant_code(float v, float s, float qmax, float 
     return rintf(fminf(fmaxf(t, 0.f), qmax));
 }
 
+// Scratch (nn_stage_scratch_bytes): one record per channel, [ST_SPLITS][2] double partial sums (slice s: sum, sum of
+// squares) and then the channel's arrival counter, padded to 16 bytes.  Channel c's record lies at the same address
+// whatever the calling stage's C, so stages of different widths can share one scratch: a wider stage's partials never
+// cover a narrower stage's counters.
+constexpr int ST_REC = ST_SPLITS * 2 + 2;       // doubles per channel record
+__device__ __forceinline__ double* stage_rec(double* scratch, int c) { return scratch + (int64_t)c * ST_REC; }
+
 // The per-channel reductions end in the LAST slice's block of each channel (a self-resetting arrival counter behind the
 // partials): it adds the slices in fixed order -- deterministic whichever block happens to be last -- and writes the
 // statistics, so no separate finalize launch sits on the step's critical path.
-__device__ __forceinline__ bool stage_last_slice(unsigned* counters, int c, int slices) {
+__device__ __forceinline__ bool stage_last_slice(double* rec, int slices) {
+    unsigned* counter = reinterpret_cast<unsigned*>(rec + ST_SPLITS * 2);
     __threadfence();                                   // this block's partial is visible before its arrival
-    const unsigned done = atomicAdd(counters + c, 1u);
+    const unsigned done = atomicAdd(counter, 1u);
     if (done != (unsigned)slices - 1u) return false;
-    counters[c] = 0u;                                  // ready for the next launch that uses this scratch
+    *counter = 0u;                                     // ready for the next launch that uses this scratch
     __threadfence();
     return true;
 }
 
 // ------------------------------------------------------------------ F1: 2x2 max pool + per-channel partial sums
-// grid (C, ST_SPLITS); block 256.  y [B,C,OH,OW] -> pooled [B,C,PH,PW], argmax (0..3), partial [C][SPLITS][2] (double)
+// grid (C, slices); block 256.  y [B,C,OH,OW] -> pooled [B,C,PH,PW], argmax (0..3), partial sums in the channel records
 __global__ void __launch_bounds__(256)
-k_pool_stats(const float* __restrict__ y, float* __restrict__ pooled, uint8_t* __restrict__ amax, double* __restrict__ partial,
-             unsigned* __restrict__ counters, const BnFinP fin, int B, int C, int OH, int OW) {
+k_pool_stats(const float* __restrict__ y, float* __restrict__ pooled, uint8_t* __restrict__ amax, double* __restrict__ scratch,
+             const BnFinP fin, int B, int C, int OH, int OW) {
     const int c = blockIdx.x, sp = blockIdx.y;
     if (c == 0 && sp == 0 && threadIdx.x == 0 && fin.xmax_out) *fin.xmax_out = 0.f;      // the pack kernel that follows maxes into it
     const int PH = OH >> 1, PW = OW >> 1, PHW = PH * PW;
@@ -94,16 +102,16 @@ k_pool_stats(const float* __restrict__ y, float* __restrict__ pooled, uint8_t* _
     if (threadIdx.x == 0) {
         double a = 0, b = 0;
         for (int w = 0; w < 8; ++w) { a += sh[0][w]; b += sh[1][w]; }
-        partial[((int64_t)c * gridDim.y + sp) * 2 + 0] = a;
-        partial[((int64_t)c * gridDim.y + sp) * 2 + 1] = b;
-        if (stage_last_slice(counters, c, (int)gridDim.y)) bn_finalize_channel(partial + (int64_t)c * gridDim.y * 2, (int)gridDim.y, 2, c, fin);
+        double* rec = stage_rec(scratch, c);
+        rec[sp * 2 + 0] = a;
+        rec[sp * 2 + 1] = b;
+        if (stage_last_slice(rec, (int)gridDim.y)) bn_finalize_channel(rec, (int)gridDim.y, 2, c, fin);
     }
 }
 
 // statistics only (fc stages / no pooling): x [B,C,HW]
 __global__ void __launch_bounds__(256)
-k_chan_stats(const float* __restrict__ x, double* __restrict__ partial, unsigned* __restrict__ counters, const BnFinP fin,
-             int B, int C, int HW) {
+k_chan_stats(const float* __restrict__ x, double* __restrict__ scratch, const BnFinP fin, int B, int C, int HW) {
     const int c = blockIdx.x, sp = blockIdx.y;
     if (c == 0 && sp == 0 && threadIdx.x == 0 && fin.xmax_out) *fin.xmax_out = 0.f;
     const int b0 = (int)((int64_t)B * sp / (int)gridDim.y), b1 = (int)((int64_t)B * (sp + 1) / (int)gridDim.y);
@@ -137,9 +145,10 @@ k_chan_stats(const float* __restrict__ x, double* __restrict__ partial, unsigned
     if (threadIdx.x == 0) {
         double a = 0, b = 0;
         for (int w = 0; w < 8; ++w) { a += sh[0][w]; b += sh[1][w]; }
-        partial[((int64_t)c * gridDim.y + sp) * 2 + 0] = a;
-        partial[((int64_t)c * gridDim.y + sp) * 2 + 1] = b;
-        if (stage_last_slice(counters, c, (int)gridDim.y)) bn_finalize_channel(partial + (int64_t)c * gridDim.y * 2, (int)gridDim.y, 2, c, fin);
+        double* rec = stage_rec(scratch, c);
+        rec[sp * 2 + 0] = a;
+        rec[sp * 2 + 1] = b;
+        if (stage_last_slice(rec, (int)gridDim.y)) bn_finalize_channel(rec, (int)gridDim.y, 2, c, fin);
     }
 }
 
@@ -363,8 +372,7 @@ k_bn_act_pack_tiled(const BnActP p) {
 // ------------------------------------------------------------------ B1: masks + per-channel sums of dv, dv*xhat
 struct BnBwdP {
     const float *g, *x, *mean, *invstd, *gamma, *beta;
-    double* partial;              // [C][SPLITS][2]
-    unsigned* counters;           // [C] arrivals (self-resetting)
+    double* scratch;              // channel records: partial sums + arrival counter (self-resetting)
     float *dbeta, *dgamma;        // written by the last slice's block of each channel
     int B, C, HW;
     float act_max, q_hi;
@@ -436,12 +444,13 @@ k_bn_bwd_stats(const BnBwdP p) {
     if (threadIdx.x == 0) {
         double a = 0, b = 0;
         for (int w = 0; w < 8; ++w) { a += sh[0][w]; b += sh[1][w]; }
-        p.partial[((int64_t)c * gridDim.y + sp) * 2 + 0] = a;
-        p.partial[((int64_t)c * gridDim.y + sp) * 2 + 1] = b;
-        if (stage_last_slice(p.counters, c, (int)gridDim.y)) {
+        double* rec = stage_rec(p.scratch, c);
+        rec[sp * 2 + 0] = a;
+        rec[sp * 2 + 1] = b;
+        if (stage_last_slice(rec, (int)gridDim.y)) {
             const int splits = (int)gridDim.y;
             double s1 = 0, s2 = 0;
-            for (int s = 0; s < splits; ++s) { s1 += __ldcg(p.partial + ((int64_t)c * splits + s) * 2); s2 += __ldcg(p.partial + ((int64_t)c * splits + s) * 2 + 1); }
+            for (int s = 0; s < splits; ++s) { s1 += __ldcg(rec + s * 2); s2 += __ldcg(rec + s * 2 + 1); }
             p.dbeta[c] = (float)s1;        // grads are OVERWRITTEN (the step zeroes them anyway)
             p.dgamma[c] = (float)s2;
         }
@@ -1159,8 +1168,8 @@ static inline int grid_cap(int64_t items, int device, int waves = 8) {
 
 }  // namespace
 
-// [C][ST_SPLITS][2] double partial sums, then [C] arrival counters
-extern "C" int64_t nn_stage_scratch_bytes(int C) { return (int64_t)C * ST_SPLITS * 2 * sizeof(double) + (int64_t)((C + 3) / 4 * 4) * sizeof(unsigned); }
+// C channel records (stage_rec): monotone in C, so one scratch sized for the widest stage serves every stage
+extern "C" int64_t nn_stage_scratch_bytes(int C) { return (int64_t)C * ST_REC * sizeof(double); }
 
 extern "C" int nn_stage_fwd(const nn_stage_args* a, int device, void* stream) {
     if (!a || !a->in || !a->xp || !a->scratch || !a->mean || !a->invstd)
@@ -1176,8 +1185,7 @@ extern "C" int nn_stage_fwd(const nn_stage_args* a, int device, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     const float* bn_in = a->in;
     int HW = a->H * a->W;
-    double* partial = (double*)a->scratch;
-    unsigned* counters = (unsigned*)(partial + (size_t)a->C * ST_SPLITS * 2);
+    double* scratch = (double*)a->scratch;
     int splits = ST_SPLITS;
     BnFinP fin;
     fin.eps = a->eps; fin.momentum = a->momentum; fin.mean = a->mean; fin.invstd = a->invstd; fin.running_mean = a->running_mean;
@@ -1191,14 +1199,14 @@ extern "C" int nn_stage_fwd(const nn_stage_args* a, int device, void* stream) {
         splits = stage_splits((int64_t)a->B * HW);
         dim3 grid(a->C, splits);
         fin.count = (double)a->B * HW;
-        k_pool_stats<<<grid, 256, 0, st>>>(a->in, a->pooled, a->argmax, partial, counters, fin, a->B, a->C, a->H, a->W);
+        k_pool_stats<<<grid, 256, 0, st>>>(a->in, a->pooled, a->argmax, scratch, fin, a->B, a->C, a->H, a->W);
         NN_LAUNCH_OK();
         bn_in = a->pooled;
     } else {
         splits = stage_splits((int64_t)a->B * HW);
         dim3 grid(a->C, splits);
         fin.count = (double)a->B * HW;
-        k_chan_stats<<<grid, 256, 0, st>>>(a->in, partial, counters, fin, a->B, a->C, HW);
+        k_chan_stats<<<grid, 256, 0, st>>>(a->in, scratch, fin, a->B, a->C, HW);
         NN_LAUNCH_OK();
     }
     BnActP p;
@@ -1241,7 +1249,7 @@ extern "C" int nn_stage_bwd(const nn_stage_bwd_args* a, int device, void* stream
     const int PH = a->pool ? a->H / 2 : a->H, PW = a->pool ? a->W / 2 : a->W;
     BnBwdP q;
     q.g = a->g; q.x = a->x; q.mean = a->mean; q.invstd = a->invstd; q.gamma = a->gamma; q.beta = a->beta;
-    q.partial = (double*)a->scratch; q.counters = (unsigned*)(q.partial + (size_t)a->C * ST_SPLITS * 2);
+    q.scratch = (double*)a->scratch;
     q.dbeta = a->dbeta; q.dgamma = a->dgamma; q.B = a->B; q.C = a->C; q.HW = PH * PW; q.act_max = a->act_max;
     q.q_hi = a->q_bits > 0 ? (float)a->q_hi : 0.f;
     q.keep = drop ? a->keep : nullptr; q.drop_k = drop ? 1.0f / (float)(1.0 - a->drop_p) : 1.0f;
