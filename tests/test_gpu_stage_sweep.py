@@ -153,33 +153,36 @@ def test_scratch_layout_matches_library(lib):
 
 # ---------------------------------------------------------------------------------------------- references
 
-def _philox_u(B, C_, HW):
+def _philox_u(B, C_, HW, seed=SEED, offset=OFFSET, stoch=STOCH):
     """the stochastic-rounding draws of thread i = pixel * Cp/8 + chunk: channel c reads group 2i + (c % 8) / 4, word
     c % 4; u = fl(fl(u01(r) * fl(2s)) - s).  [B, C, HW] float32"""
     from oracle.noisynet_oracle import philox4x32_10
     chunks = _pad8(C_) // 8
     i = np.arange(B * HW * chunks, dtype=np.uint64)
     g = np.stack([2 * i, 2 * i + 1], axis=-1)                             # [threads, 2]
-    r = philox4x32_10(g, SEED, OFFSET).reshape(B * HW, chunks * 8)[:, :C_]
+    r = philox4x32_10(g, seed, offset).reshape(B * HW, chunks * 8)[:, :C_]
     u01 = (r >> np.uint32(8)).astype(np.float32) * np.float32(2.0 ** -24)
-    u = (u01 * np.float32(2.0 * STOCH)).astype(np.float32) - np.float32(STOCH)
+    u = (u01 * np.float32(2.0 * stoch)).astype(np.float32) - np.float32(stoch)
     return np.ascontiguousarray(u.reshape(B, HW, C_).transpose(0, 2, 1))
 
 
-def _v(x, mean, invstd, gamma, beta):
+def _v(x, mean, invstd, gamma, beta, fma=False):
     """fl(fl(fl(x - mean) * invstd) * gamma + beta), per channel (axis 1 of [B, C, HW]); exact for power-of-two gamma
-    whether or not the kernel contracts the last two operations into an FMA"""
+    whether or not the kernel contracts the last two operations into an FMA.  fma=True: the contracted form
+    fl(xhat * gamma + beta) with one rounding (the product is exact in float64)"""
     e = lambda a: a.astype(np.float32)[None, :, None]
     xhat = ((x - e(mean)) * e(invstd)).astype(np.float32)
+    if fma:
+        return xhat, (xhat.astype(np.float64) * e(gamma).astype(np.float64) + e(beta).astype(np.float64)).astype(np.float32)
     return xhat, (xhat * e(gamma) + e(beta)).astype(np.float32)
 
 
-def _codes(x, mean, invstd, gamma, beta, u):
+def _codes(x, mean, invstd, gamma, beta, u, act_max=ACT_MAX, q_scale=Q_SCALE, qmax=QMAX, fma=False):
     """ReLU, clamp, then rint(clip(fl(fl(v / s) + u), 0, qmax)), all in float32"""
-    _, v = _v(x, mean, invstd, gamma, beta)
-    v = np.minimum(np.maximum(v, np.float32(0)), np.float32(ACT_MAX))
-    t = (v / Q_SCALE).astype(np.float32) + u.astype(np.float32)
-    return np.rint(np.clip(t, np.float32(0), QMAX))
+    _, v = _v(x, mean, invstd, gamma, beta, fma)
+    v = np.minimum(np.maximum(v, np.float32(0)), np.float32(act_max))
+    t = (v / np.float32(q_scale)).astype(np.float32) + u.astype(np.float32)
+    return np.rint(np.clip(t, np.float32(0), np.float32(qmax)))
 
 
 def _slice_sums(a, splits):
@@ -414,10 +417,10 @@ def _bwd_operands(B, C_, PH, PW, pool, gen):
     return x.float(), g, amax, mean.float(), invstd.float(), gamma.float(), beta.float()
 
 
-def _bwd_reference(x, g, mean, invstd, gamma, beta, act_max, q_hi):
+def _bwd_reference(x, g, mean, invstd, gamma, beta, act_max, q_hi, fma=False):
     """the STE / clamp / ReLU masks (pass iff v > 0, v <= act_max, min(v, act_max) <= q_hi), and dv, xhat"""
     B, C_ = x.shape[:2]
-    xhat, v = _v(x.reshape(B, C_, -1), mean, invstd, gamma, beta)
+    xhat, v = _v(x.reshape(B, C_, -1), mean, invstd, gamma, beta, fma)
     keep = (v > 0) & (v <= np.float32(act_max)) & (np.minimum(v, np.float32(act_max)) <= np.float32(q_hi))
     return np.where(keep, g.reshape(B, C_, -1), np.float32(0)), xhat, v
 
